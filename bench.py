@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the GGUF dequant hot path on B200 (BASELINE.json metric "dequant GB/s vs HBM peak").
+"""bench.py -- headline benchmark of the GGUF dequant hot path on H100 (BASELINE.json metric "dequant GB/s vs HBM peak").
 
 Workload (BASELINE.json configs[1]): standalone dequant sweep Q4_0 / Q4_K / Q5_K / Q6_K / Q8_0 over the seven
 Flux.1-dev Linear weight shapes, fp16 output, reference-default fp16 math.  One STEP = one pass over all 35 packed
 tensors (35 kernel launches, 1.42 G elements, 1.05 GB packed read + 2.83 GB written).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 value      algorithmic GB/s (packed bytes read + output bytes written) / device time, inputs resident in HBM
 e2e        same metric and the same 35 tensors through the plugin call (`dequantize_tensor`) with HOST buffers: pinned-host
@@ -16,6 +16,9 @@ cpu_baseline  the C oracle port of the reference algorithm on the host cores (bo
 N > 1      independent replicas (one process per GPU, torchrun), no collective on the data path; value = sum of
            units / max-over-ranks device time  ("scaling": "weak")
 --impl reference   times the reference's CPU algorithm (oracle port, all host threads) on the same 35 tensors per step
+--dump-outputs DIR after the timed steps, writes what the last timed step computed: for each of the 35 tensors a fixed, seeded
+           sample of 2^17 elements of its fp16 output, as DIR/<qtype>_<N>x<K>.npy (float32, 18 MB in all).  The inputs are
+           seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -47,7 +50,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def host_threads():
@@ -194,39 +197,21 @@ def cpu_baseline_run(budget_s=12.0, threads=None):
         tot_s += med
     res["numpy_gguf_py"] = {"value": tot_bytes / tot_s / 1e9, "unit": UNIT, "cores": 1, "per_qtype": per_q,
                             "sample": f"gguf.quants.dequantize [3072,3072] -> fp32 for each of {'/'.join(QTYPES)}, median of 5 after 1 warm-up"}
-    # the reference's own torch path on CPU tensors (dequant.py::dequantize_tensor), when the reference checkout is present
-    # (this container; it does not travel to the GPU box)
-    ref_py = "/root/reference/dequant.py"
-    if os.path.exists(ref_py):
-        try:
-            import importlib.util
-            import torch
-            spec = importlib.util.spec_from_file_location("ref_dequant_bench", ref_py)
-            refdq = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(refdq)
-            per_q, tot_bytes, tot_s = {}, 0.0, 0.0
-            for q, code, raw in tensors:
-                qt = gguf.GGMLQuantizationType(code)
-                data = torch.from_numpy(raw.reshape(N, -1))
-                refdq.dequantize(data, qt, (N, K), dtype=None)
-                ts_ = []
-                for _ in range(5):
-                    t1 = time.perf_counter()
-                    refdq.dequantize(data, qt, (N, K), dtype=None)
-                    ts_.append(time.perf_counter() - t1)
-                med = float(np.median(ts_))
-                b = alg_bytes(q, N * K)
-                per_q[q] = b / med / 1e9
-                tot_bytes += b
-                tot_s += med
-            res["torch_cpu_reference"] = {"value": tot_bytes / tot_s / 1e9, "unit": UNIT, "cores": torch.get_num_threads(), "per_qtype": per_q,
-                                          "kind": "reference", "sample": "the unmodified /root/reference/dequant.py::dequantize on CPU tensors "
-                                          f"[3072,3072] for each of {'/'.join(QTYPES)}, fp16 math, median of 5 after 1 warm-up"}
-        except Exception as exc:
-            res["torch_cpu_reference"] = {"unavailable": repr(exc)[:160]}
-    else:
-        res["torch_cpu_reference"] = {"unavailable": "/root/reference is not present on this box (GPU box); see profiles/ for the container run"}
     return res
+
+
+DUMP_SAMPLE = 1 << 17
+
+
+def dump_outputs(out_dir, tensors):
+    """The fp16 output of every tensor of the last timed step: a fixed, seeded sample of DUMP_SAMPLE elements each, as float32."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for i, t in enumerate(tensors):
+        flat = t["out"].reshape(-1)
+        idx = np.sort(np.random.default_rng(1000 + i).choice(flat.numel(), size=min(DUMP_SAMPLE, flat.numel()), replace=False))
+        vals = flat[torch.from_numpy(idx).to(flat.device)].float().cpu().numpy()
+        np.save(os.path.join(out_dir, f"{t['q']}_{t['shape'][0]}x{t['shape'][1]}.npy"), vals.astype(np.float32))
 
 
 def run_reference(args):
@@ -294,6 +279,7 @@ def main():
     ap.add_argument("--eager", action="store_true", help="time eager launches instead of replaying each step from a CUDA graph")
     ap.add_argument("--sweep-detail", action="store_true", help="also print per-(qtype,shape) GB/s lines to stderr")
     ap.add_argument("--no-flux", action="store_true", help="skip the secondary metric (Flux.1-shape Q4_K denoise step A/B)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a seeded sample of every output of the last timed step to DIR/*.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -401,6 +387,8 @@ def main():
     torch.cuda.synchronize()
     rep.barrier()
     local_ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, tensors)
     total_ms = rep.max_over_ranks(local_ms)
     total_bytes = rep.sum_over_ranks(float(step_bytes) * args.steps)
     value = total_bytes / (total_ms * 1e-3) / 1e9
@@ -479,17 +467,6 @@ def main():
                 "note": "achieved = mean algorithmic bytes per launch / (CUDA-event time of the timed region / launches in it); "
                         "the timed region contains only this kernel (35 launches per step, "
                         + ("eager" if args.eager else "CUDA-graph replay") + ", programmatic dependent launch)"}
-    traffic_file = os.path.join(ROOT, "profiles", "dequant_traffic.json")
-    if os.path.exists(traffic_file):
-        try:
-            tf = json.load(open(traffic_file))
-            pl = tf["per_launch"]
-            roofline["traffic"] = sum(x["dram_read_bytes"] + x["dram_write_bytes"] for x in pl) / len(pl)
-            roofline["traffic_algorithmic_same_launches"] = sum(x["algorithmic_read_bytes"] + x["algorithmic_write_bytes"] for x in pl) / len(pl)
-            roofline["traffic_unit"] = "bytes per launch (mean over the 7 Q4_K launches of one ncu --set full capture)"
-            roofline["traffic_note"] = tf["note"]
-        except Exception:
-            pass
 
     # ---------------- e2e through the plugin call with HOST buffers
     e2e = None
@@ -568,7 +545,7 @@ def main():
             "config": {"workload": WORKLOAD, "tensors_per_step": n_tensors, "elements_per_step": step_elems,
                        "algorithmic_bytes_per_step": step_bytes, "parallelism": f"{world} independent replica(s), no collective",
                        "launch": "ggufb200_dequant(..., math_dtype = fp16" + ("" if args.no_src_stable else " | GGUFB200_DEQUANT_SRC_STABLE") + ")",
-                       "l2": "inputs larger than L2: 1.05 GB of distinct packed tensors + 2.83 GB of distinct outputs per step vs 126 MB L2"},
+                       "l2": "inputs larger than L2: 1.05 GB of distinct packed tensors + 2.83 GB of distinct outputs per step vs 50 MB L2"},
             "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": launches, "clocks": clocks, "flux_step": flux,
             "numa": numa,
         }))

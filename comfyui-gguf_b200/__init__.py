@@ -1,4 +1,4 @@
-"""ggufb200: B200-native (sm_100a) drop-in for the dequant + Linear hot path of city96/ComfyUI-GGUF.
+"""ggufb200: H100-native (sm_90a) drop-in for the dequant + Linear hot path of city96/ComfyUI-GGUF.
 
 ComfyUI imports this directory as a custom node package and reads NODE_CLASS_MAPPINGS / NODE_DISPLAY_NAME_MAPPINGS from it.
 Outside ComfyUI (tests, benchmarks, the GPU box) the host packages are absent and only the kernel-facing modules

@@ -28,7 +28,7 @@ class GGUFB200Error(RuntimeError):
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the CUDA sources in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile the CUDA sources in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     out = subprocess.run(["bash", os.path.join(_HERE, "csrc", "build.sh")], capture_output=True, text=True)
     if verbose or out.returncode != 0:
         print(out.stdout, out.stderr)

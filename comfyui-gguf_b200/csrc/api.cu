@@ -19,7 +19,7 @@ int gemm2_fused_dispatch(int type, const void *W, long long N, long long K, cons
                          int math_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes, int flags,
                          cudaStream_t st);
 int gemm2_fused_splits(long long M, long long N, long long K);
-void gemm2_fused_plan_info(long long M, long long N, long long K, size_t ws_bytes, int flags, int *accs, int *splits, int *kb_per_split, int *ctas);
+void gemm2_fused_plan_info(long long M, long long N, long long K, size_t ws_bytes, int flags, int *tile_rows, int *splits, int *kb_per_split, int *ctas);
 int gemm3_dense_dispatch(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx,
                          int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st);
 int gemm4_fused_dispatch(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
@@ -67,11 +67,11 @@ static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 
 static bool fused_type(int t) { return t != T_BF16 && type_geom(t, nullptr, nullptr); }     // every block format has a fused producer
 
 // ------------------------------------------------------------------ device gate
-// The library contains sm_100a code only.  Checked once per device, right before the first launch on it (argument
+// The library contains sm_90a code only.  Checked once per device, right before the first launch on it (argument
 // errors are still reported without a GPU).
 static int device_check()
 {
-    static signed char ok[64] = {};     // 0 = unknown, 1 = sm_100, -1 = something else
+    static signed char ok[64] = {};     // 0 = unknown, 1 = sm_90, -1 = something else
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) {
         cudaGetLastError();
@@ -85,24 +85,12 @@ static int device_check()
             cudaGetLastError();
             return GGUFB200_E_CUDA;
         }
-        ok[dev] = (major == 10 && minor == 0) ? 1 : -1;
+        ok[dev] = (major == 9 && minor == 0) ? 1 : -1;
     }
     return ok[dev] == 1 ? GGUFB200_OK : GGUFB200_E_DEVICE;
 }
 
 // ------------------------------------------------------------------ route selection
-// Fallback thresholds (round 1) for weights the TMEM-fed kernel cannot stage: short activations split-K fused through shared
-// memory, long activations dequant once into the workspace + dense tcgen05 GEMM.
-static bool exact_prefers_fused(long long M, long long N, long long K)
-{
-    if ((K % 64) != 0) return false;
-    if (M > 1024) return false;
-    const int splits = gemm2_fused_splits(M, N, K);
-    if (splits >= 4 || (splits >= 2 && K >= 2 * N)) return true;
-    if (splits >= 2) return false;
-    return M > 256 && N >= 12288;
-}
-
 struct Route {
     int algo;          // GGUFB200_ALGO_* without flags
     size_t ws;         // workspace bytes the route wants (0 = none)
@@ -139,17 +127,21 @@ static Route pick_route(int type, const void *W, long long M, long long N, long 
     const bool fusable = fused_type(type) && math == kF16 && (K % 64) == 0 && (N % 8) == 0;
     Route r{algo, 0};
     if (algo == GGUFB200_ALGO_AUTO) {
-        // Measured on B200 (profiles/r02_bench_linear_*.log, r02_bench_gemv*.log).  The TMEM-fed fused kernel is the route for
-        // every M > 8 (with EXACT_W it runs the reference-sequence producers at the same speed: it is tensor-pipe bound) and for
-        // M <= 8 on large weights; the mma.sync GEMV keeps small weights at M <= 8 (its fixed cost is lower).  A math dtype other
-        // than fp16 means the reference's own sequence in that dtype: standalone dequant + dense GEMM (or the GEMV).
+        // Measured on an H100 80GB HBM3 (400 W power limit, Q4_K / Q6_K at Flux shapes, tools/bench_linear.py --graph):
+        //  * M <= 8: the mma.sync GEMV takes 0.35-0.56 of FUSED_TMEM's time on every weight up to 21504 x 3072, so it serves all
+        //    of them (the integer-pattern GEMV when the caller allows the `fast` contract);
+        //  * M > 8: the FUSED_TMEM kernel;
+        //  * weights that kernel cannot read (no span-major copy at hand): dequant once + the dense GEMM took 0.18-0.89 of the
+        //    fused reference-exact kernel's time at every M from 64 to 4608, so FUSED_MMA is only taken when the caller's
+        //    workspace cannot hold the dequantised weight.
+        // A math dtype other than fp16 means the reference's own sequence in that dtype: standalone dequant + dense GEMM (or the GEMV).
         const bool tmem_ok = w_ok && fused_type(type) && math == kF16 && (N % 8) == 0 && (have_spans || gemm4_supported(type, W, N, K));
         const bool exact = (flags & GGUFB200_FLAG_EXACT_W) != 0 || math != kF16;
         if (!w_ok) r.algo = GGUFB200_ALGO_DEQUANT_MMA;
         else if (M <= gemv_max_m() && !exact && gemv2_supported(type, W ? W : (const void *)16, N, K, M)) r.algo = GGUFB200_ALGO_GEMV_FAST;
-        else if (M <= gemv_max_m()) r.algo = (tmem_ok && (long long)N * K >= (40ll << 20)) ? GGUFB200_ALGO_FUSED_TMEM : GGUFB200_ALGO_GEMV;
+        else if (M <= gemv_max_m()) r.algo = GGUFB200_ALGO_GEMV;
         else if (tmem_ok) r.algo = GGUFB200_ALGO_FUSED_TMEM;
-        else if (fusable && (exact_prefers_fused(M, N, K) || ws_avail < dense)) r.algo = GGUFB200_ALGO_FUSED_MMA;
+        else if (fusable && ws_avail < dense) r.algo = GGUFB200_ALGO_FUSED_MMA;
         else r.algo = GGUFB200_ALGO_DEQUANT_MMA;
     }
     switch (r.algo) {
@@ -178,7 +170,7 @@ const char *ggufb200_strerror(int rc)
     case GGUFB200_E_CUDA: return "CUDA launch failed";
     case GGUFB200_E_WORKSPACE: return "workspace too small (see ggufb200_linear_workspace)";
     case GGUFB200_E_UNSUPPORTED: return "operation not implemented for this type / dtype / shape combination";
-    case GGUFB200_E_DEVICE: return "current CUDA device is not sm_100 (B200)";
+    case GGUFB200_E_DEVICE: return "current CUDA device is not sm_90 (H100)";
     }
     return "unknown error";
 }
@@ -303,7 +295,7 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
     if (!aligned16(X) || (ldx % 8) != 0) return GGUFB200_E_ALIGN;
     if (vec_y && (!aligned16(Y) || (ldy % 8) != 0)) return GGUFB200_E_ALIGN;
     if (workspace && !aligned16(workspace) && r.ws) return GGUFB200_E_ALIGN;
-    if (lora) {     // the rank-r update rides as one extra k-block of the TMEM-fed kernel: no other route can carry it
+    if (lora) {     // the rank-r update rides as one extra k-block of the FUSED_TMEM kernel: no other route can carry it
         if (r.algo != GGUFB200_ALGO_FUSED_TMEM) return GGUFB200_E_UNSUPPORTED;
         if (!lora->T || !lora->U) return GGUFB200_E_NULL;
         if (!aligned16(lora->T) || !aligned16(lora->U) || lora->ldt < 64 || (lora->ldt % 8) != 0) return GGUFB200_E_ALIGN;
@@ -321,7 +313,6 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
         if (!fused_type(ggml_type)) return GGUFB200_E_UNSUPPORTED;
         int f = 0;
         if (flags & GGUFB200_FLAG_NOSPLIT) f |= 1;
-        if (flags & GGUFB200_FLAG_UNSTAGED) f |= 2;
         return gemm2_fused_dispatch(ggml_type, W_packed, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, workspace,
                                     ws_avail, f, st);
     }
@@ -400,9 +391,7 @@ int ggufb200_linear_plan(int ggml_type, int64_t M, int64_t N, int64_t K, size_t 
         return GGUFB200_OK;
     }
     if ((algo & GGUFB200_ALGO_MASK) != GGUFB200_ALGO_FUSED_MMA) return GGUFB200_E_UNSUPPORTED;
-    int accs = 1;
-    gemm2_fused_plan_info(M, N, K, workspace_bytes, (flags & GGUFB200_FLAG_NOSPLIT) ? 1 : 0, &accs, k_ranges, kblocks_per_range, ctas);
-    *tile_rows = 256 * accs;
+    gemm2_fused_plan_info(M, N, K, workspace_bytes, (flags & GGUFB200_FLAG_NOSPLIT) ? 1 : 0, tile_rows, k_ranges, kblocks_per_range, ctas);
     return GGUFB200_OK;
 }
 

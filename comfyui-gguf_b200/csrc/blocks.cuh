@@ -2,7 +2,7 @@
 //
 // One struct per ggml type (the keys of the reference's dispatch table, dequant.py:287-301).
 // Every struct exposes the same interface so the standalone dequant kernel, the row-gather
-// kernel, the fused GEMV and the fused tcgen05 GEMM all share one unpack implementation:
+// kernel, the fused GEMV and the fused warpgroup-MMA GEMM all share one unpack implementation:
 //
 //   BS, TS      block size (elements) and type size (bytes)          gguf-py GGML_QUANT_SIZES
 //   BIAS        q4() returns u = q + BIAS as unsigned bytes (q = integer entering the multiply)

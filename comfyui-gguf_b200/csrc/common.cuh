@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for libggufb200 (sm_100a only).
+// common.cuh -- shared device helpers for libggufb200 (sm_90a only).
 //
 //  * PTX wrappers: mbarrier, 1-D bulk async copy (TMA engine, SASS UBLKCP), vector ld/st
 //  * "math policies": the reference (dequant.py) runs every float op as its own torch
@@ -281,20 +281,20 @@ template <class Kernel> inline bool ensure_dynamic_smem(Kernel kern, int bytes, 
 }
 
 // SM count of the current device, queried once per device (the attribute call is a driver round trip that showed up in the
-// host cost of short-activation Linears).  148 when no device is visible (ABI tests on a CPU-only box).
+// host cost of short-activation Linears).  132 (an H100 SXM) when no device is visible (plan tests without a GPU).
 inline int sm_count()
 {
     static int cache[64] = {};
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
         cudaGetLastError();
-        return 148;
+        return 132;
     }
     if (cache[dev] == 0) {
-        int sms = 148;
+        int sms = 132;
         if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) {
             cudaGetLastError();
-            sms = 148;
+            sms = 132;
         }
         cache[dev] = sms;
     }

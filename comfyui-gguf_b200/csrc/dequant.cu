@@ -9,16 +9,14 @@
 //     into tiles of 4096 elements whose byte span is always a multiple of 16 B
 //   * ONE TILE PER CTA (128 threads), CTAs handed out by the hardware in address order: the write front stays
 //     compact, an SM that happens to be slower simply takes fewer tiles, and 16 CTAs per SM cover each other's load
-//     latency.  (Round 1's persistent CTAs with a 3-stage prefetch ring and strided tiles: 0.885 of the measured copy peak
-//     on the Flux-shape sweep, 5.8 TB/s on a 1 GB output; this form: 0.949 and 6.75 TB/s --
-//     profiles/r02_k1_variants_ab.log, same effect as in tools/probe_write.cu's plain-store probes.)
+//     latency (instead of persistent CTAs walking strided tiles through a prefetch ring, whose write fronts spread out).
 //   * the tile is staged into shared memory by thread 0 with the TMA engine (cp.async.bulk, SASS UBLKCP), completion on
 //     an mbarrier that only thread 0 polls; the other threads sleep in the CTA barrier
 //   * every thread unpacks one run of 32 consecutive elements from shared memory (blocks.cuh) into its row of the output
 //     tile in shared memory, which leaves through ONE swizzled tensor-map store (cp.async.bulk.tensor.2d, SASS UTMASTG): no
 //     thread computes a global address, every HBM write is a full line, and the unpack runs with immediate offsets
 #include "blocks.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ggufb200 {
 
@@ -38,8 +36,8 @@ __device__ __forceinline__ void st_otile_v4(uint32_t saddr, uint32_t a, uint32_t
 // a swizzled 2-D tensor-map store, one row per thread (fp16 / bf16: 64-byte rows, CU_TENSOR_MAP_SWIZZLE_64B; fp32: 128-byte rows,
 // SWIZZLE_128B): 16-byte chunk p of a row sits at chunk p ^ (address bits 7.. of the row), so the chunks are processed in their
 // natural order -- every byte offset and shift of the unpack is an immediate -- and the STS.128 of a quarter-warp still hit eight
-// different bank groups.  (A linear tile needs the chunk ORDER rotated per lane instead: dynamic offsets and shifts, 7-17 % more
-// instructions, 0.951 instead of 0.997 of the copy peak on the Flux-shape sweep -- profiles/r02_k1_variants_ab.log.)
+// different bank groups.  (A linear tile needs the chunk ORDER rotated per lane instead: dynamic offsets and shifts, more
+// instructions.)
 template <class Q, int MATH, int OUT>
 __device__ __forceinline__ void dequant_tile(const uint8_t *tile, uint8_t *otile, int tile_elems, int tid)
 {

@@ -35,7 +35,7 @@ template <int ACT> __device__ __forceinline__ float load_bias(const void *bias, 
 
 // ------------------------------------------------------------------ tensor-core variant (default)
 // The dot products of 16 output features x up to 8 activation rows are one mma.sync.m16n8k16 tile (legacy HMMA path: the
-// kernel is bound by the weight stream, not by flops; tcgen05 needs M = 128 lanes and would idle 94 % of them here).
+// kernel is bound by the weight stream, not by flops; a warpgroup MMA needs M = 64 rows and would idle most of them here).
 // A = dequantised W (16 features x 16 k), B = X^T (16 k x 8 rows), D = fp32 16 x 8.  The k index of a dot product may be
 // permuted freely as long as A and B use the same permutation, so thread (g = lane/4, c = lane%4) simply owns the run of 32
 // consecutive k  [128*span + 32c, +32)  of rows g and g+8 (header decoded once per run) and of activation row g: every
@@ -76,6 +76,9 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_mma_kernel(const uint8_t *_
         const uint8_t *w1 = W + (ok1 ? n0 + g + 8 : 0) * row_bytes;
         float d[4] = {0.f, 0.f, 0.f, 0.f};
         for (long long span = warp; span < n_spans; span += kGemvThreads / 32) {
+            // the tensor cores accumulate one span (8 MMAs) into fresh registers; spans are summed with round-to-nearest fp32
+            // adds, so a long K never runs as one chain of tensor-core accumulations (their additions are not rounded to nearest)
+            float sp[4] = {0.f, 0.f, 0.f, 0.f};
             // K % 32 == 0, so a run is entirely inside or outside; lanes whose run is past K must still execute the
             // warp-wide mma.sync, so they contribute zero fragments instead of skipping
             const long long kreal = span * 128 + c * 32;
@@ -97,8 +100,8 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_mma_kernel(const uint8_t *_
                         for (int t = 0; t < 2; ++t) {
                             uint4 xv = make_uint4(0, 0, 0, 0);
                             if (xrow_ok) xv = *reinterpret_cast<const uint4 *>(xrow + (k + hseg * 16 + t * 8) * 2);
-                            mma_16x8x16<ACT>(d, a[4 * t], b[4 * t], a[4 * t + 1], b[4 * t + 1], xv.x, xv.y);
-                            mma_16x8x16<ACT>(d, a[4 * t + 2], b[4 * t + 2], a[4 * t + 3], b[4 * t + 3], xv.z, xv.w);
+                            mma_16x8x16<ACT>(sp, a[4 * t], b[4 * t], a[4 * t + 1], b[4 * t + 1], xv.x, xv.y);
+                            mma_16x8x16<ACT>(sp, a[4 * t + 2], b[4 * t + 2], a[4 * t + 3], b[4 * t + 3], xv.z, xv.w);
                         }
                     } else {
 #pragma unroll
@@ -109,8 +112,8 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_mma_kernel(const uint8_t *_
                             const uint32_t a2 = (ok0 && kin) ? a[4 * t + 2] : 0u, a3 = (ok0 && kin) ? a[4 * t + 3] : 0u;
                             const uint32_t c0 = (ok1 && kin) ? b[4 * t] : 0u, c1 = (ok1 && kin) ? b[4 * t + 1] : 0u;
                             const uint32_t c2 = (ok1 && kin) ? b[4 * t + 2] : 0u, c3 = (ok1 && kin) ? b[4 * t + 3] : 0u;
-                            mma_16x8x16<ACT>(d, a0, c0, a1, c1, xv.x, xv.y);
-                            mma_16x8x16<ACT>(d, a2, c2, a3, c3, xv.z, xv.w);
+                            mma_16x8x16<ACT>(sp, a0, c0, a1, c1, xv.x, xv.y);
+                            mma_16x8x16<ACT>(sp, a2, c2, a3, c3, xv.z, xv.w);
                         }
                     }
                 }
@@ -134,10 +137,12 @@ __global__ void __launch_bounds__(kGemvThreads) gemv_mma_kernel(const uint8_t *_
                 }
                 uint4 xv = make_uint4(0, 0, 0, 0);
                 if (xrow_ok && kin) xv = *reinterpret_cast<const uint4 *>(xrow + (k + t * 8) * 2);
-                mma_16x8x16<ACT>(d, a[0], b[0], a[1], b[1], xv.x, xv.y);
-                mma_16x8x16<ACT>(d, a[2], b[2], a[3], b[3], xv.z, xv.w);
+                mma_16x8x16<ACT>(sp, a[0], b[0], a[1], b[1], xv.x, xv.y);
+                mma_16x8x16<ACT>(sp, a[2], b[2], a[3], b[3], xv.z, xv.w);
             }
             }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) d[i] += sp[i];
         }
         // d[0]: (feature g, row 2c)  d[1]: (g, 2c+1)  d[2]: (g+8, 2c)  d[3]: (g+8, 2c+1)
         part[warp][g][2 * c] = d[0];

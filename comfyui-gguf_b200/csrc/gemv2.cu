@@ -24,7 +24,7 @@
 // tiles are reduced through a double-buffered shared-memory tile at the end of a row tile (one named barrier per tile).  The
 // activations (<= 8 rows) are staged once per CTA by bulk copies, their sub-block sums computed once per CTA from that copy.
 #include "blocks.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace ggufb200 {
 
@@ -52,9 +52,10 @@ __device__ __forceinline__ void v2_bar_consumers() { asm volatile("bar.sync 1, 2
 
 __device__ __forceinline__ unsigned long long v2_fma2(unsigned long long a, unsigned long long b, unsigned long long c)
 {
-    unsigned long long r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    // two lanes of fp32 fused multiply-add, round to nearest (the operands are packed float pairs)
+    const float lo = __fmaf_rn(__uint_as_float((uint32_t)a), __uint_as_float((uint32_t)b), __uint_as_float((uint32_t)c));
+    const float hi = __fmaf_rn(__uint_as_float((uint32_t)(a >> 32)), __uint_as_float((uint32_t)(b >> 32)), __uint_as_float((uint32_t)(c >> 32)));
+    return (unsigned long long)__float_as_uint(lo) | ((unsigned long long)__float_as_uint(hi) << 32);
 }
 __device__ __forceinline__ unsigned long long v2_pack(float lo, float hi)
 {
@@ -408,7 +409,7 @@ template <int TS> static V2Plan v2_plan(long long N, long long K, long long M)
     const long long tiles = (N + 15) / 16;
     V2Plan best{false, false, 0, 0, 0};
     double best_score = 0.0;
-    for (int ctas = 2; ctas >= 1; --ctas) {          // the activations of 8 tokens + a 3-stage ring leave room for two CTAs per SM at most; three did not pay at M = 1 either (profiles/r02_bench_gemv_v3_ctas_ab.log)
+    for (int ctas = 2; ctas >= 1; --ctas) {          // the activations of 8 tokens + a 3-stage ring leave room for two CTAs per SM at most
         if (g_gemv2_ctas > 0 && ctas != g_gemv2_ctas) continue;
         const long long budget = 227 * 1024 / ctas - 1024;          // 1 KB per CTA is reserved by the system
         for (int x = 1; x >= 0; --x) {
@@ -417,7 +418,7 @@ template <int TS> static V2Plan v2_plan(long long N, long long K, long long M)
             if (ns > kV2MaxStages) ns = kV2MaxStages;
             if (ns < 3) continue;
             // makespan of the persistent grid x how well the SM hides latency with that many warps x the cost of re-reading X from L1
-            const long long grid = tiles < 148ll * ctas ? tiles : 148ll * ctas;
+            const long long grid = tiles < (long long)sm_count() * ctas ? tiles : (long long)sm_count() * ctas;
             const double rounds = (double)((tiles + grid - 1) / grid);
             const double eff = (double)tiles / (rounds * (double)grid);
             const double score = eff * (ctas == 1 ? 0.75 : 1.0) * (x ? 1.0 : (M > 2 ? 0.75 : 0.95));

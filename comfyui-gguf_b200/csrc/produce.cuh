@@ -1,8 +1,8 @@
-// produce.cuh -- W producers of the TMEM-fed fused Linear kernel (gemm4.cu): one thread turns 64 consecutive k of ONE
-// packed weight row into 32 packed fp16 pairs, ready for tcgen05.st into the A-operand columns of tensor memory.
+// produce.cuh -- W producers of the fused Linear kernels (linear_sm90.cuh): one thread turns 64 consecutive k of ONE
+// packed weight row into 32 packed fp16 pairs, ready to be stored into a swizzled shared-memory operand tile.
 //
 // `span` points at the row's packed bytes of one 256-wide K-span (eight 32-element blocks or one 256-element
-// super-block), 16-byte aligned (the kernel stages spans in shared memory with the TMA engine); `kq` = 0..3 selects
+// super-block); `kq` = 0..3 selects
 // the 64-wide quarter.  The result is delivered in two halves of 16 registers (elements 0..31 and 32..63 of the
 // quarter) through emit(half, regs) so that only 16 output registers are live at a time.
 //
@@ -13,8 +13,8 @@
 //   * FastProducer<Q>      hot formats: the sub-block products D = fp16(d*sc), M = fp16(dmin*mn) are the reference's,
 //                          the per-element step is ONE fused multiply-add fp16(D*q - M) (single rounding instead of
 //                          two: the correctly rounded value of the step), hand-scheduled loads.  The Linear stays within 1e-3 of the reference's.
-// W is handed to the tensor core as fp16 whatever the activation dtype is (kind::f16 takes A = f16 with B = bf16), so
-// no fp16 -> bf16 conversion of the weight exists in this path.
+// The kernel casts W to bf16 for bf16 activations (the cast the reference applies before F.linear): wgmma takes both
+// operands in one type.
 //
 // All functions are __host__ __device__ so tests/host_functors.cu can run them on the CPU against the oracle.
 #pragma once
@@ -32,14 +32,12 @@ template <class Q> struct SpanOf {
     static constexpr int PITCH = BYTES % 16 == 0 ? BYTES : ((PAD16 / 16) % 2 == 1 ? PAD16 : PAD16 + 16);
 };
 
-// 16-byte / 4-byte loads of a staged span.  On the device the span always lives in shared memory (gemm4.cu): say so, or
-// the compiler emits generic loads (LD.E.128 + address-space resolution) instead of LDS.128.
+// 16-byte / 4-byte loads of a row's span: the canonical rows or the span-major copy in global memory (both 16-byte aligned
+// whenever the hand-written producers are used), read through the read-only data cache.
 GG_HD uint4 ld_span16(const uint8_t *p)
 {
 #ifdef __CUDA_ARCH__
-    uint4 v;
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(smem_u32(p)));
-    return v;
+    return __ldg(reinterpret_cast<const uint4 *>(p));
 #else
     return *reinterpret_cast<const uint4 *>(p);
 #endif
@@ -47,9 +45,7 @@ GG_HD uint4 ld_span16(const uint8_t *p)
 GG_HD uint32_t ld_span4(const uint8_t *p)
 {
 #ifdef __CUDA_ARCH__
-    uint32_t v;
-    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)));
-    return v;
+    return __ldg(reinterpret_cast<const unsigned int *>(p));
 #else
     return *reinterpret_cast<const uint32_t *>(p);
 #endif
@@ -339,13 +335,5 @@ template <bool FMA> struct FastProducer<Block<T_Q6_K>, FMA> {
         }
     }
 };
-
-// ---------------------------------------------------------------- A-stage ownership of the TMEM-fed kernel (gemm4.cu)
-// The ring of A stages in tensor memory has a multiple of 4 stages and relies on ONE writer group per stage: producer group g
-// (0..3) writes exactly the k-blocks whose GLOBAL index is == g (mod 4), so the parity wait on a stage's `empty` barrier can
-// never be satisfied by a phase two uses old.  `it0` = global index of the item's first k-block (not a multiple of 4 once an
-// earlier item of this CTA pair carried a LoRA k-block).
-GG_HD int g4_group_quarter(int g, int it0) { return (g - it0) & 3; }                    // the group's quarter of every span of the item
-GG_HD int g4_lora_group(int it0, int nspans) { return (it0 + 4 * nspans) & 3; }         // the group that writes the LoRA k-block
 
 }  // namespace ggufb200

@@ -1,4 +1,4 @@
-"""Drop-in for the reference's dequant.py: same public names, B200 kernels underneath.
+"""Drop-in for the reference's dequant.py: same public names, H100 kernels underneath.
 
 Reference surface mirrored (file:line in /root/reference):
     is_torch_compatible / is_quantized       dequant.py:9-13

@@ -1,4 +1,4 @@
-"""ComfyUI graph nodes of the GGUF loader family, backed by the B200 kernels (importable only inside ComfyUI).
+"""ComfyUI graph nodes of the GGUF loader family, backed by the H100 kernels (importable only inside ComfyUI).
 
 Drop-in contract (reference nodes.py:134-321): the six node keys, their widgets, RETURN_TYPES, FUNCTION names, the
 "bootleg" category and the titles are unchanged, so saved workflows load as they are.  What the nodes hand to ComfyUI is this

@@ -1,4 +1,4 @@
-"""Drop-in for the reference's ops.py -- the ComfyUI custom-operations surface, B200 kernels inside.
+"""Drop-in for the reference's ops.py -- the ComfyUI custom-operations surface, H100 kernels inside.
 
 Mirrored surface (reference file:line):
     GGMLTensor      ops.py:44-91     tensor subclass carrying packed bytes + tensor_type/tensor_shape/patches
@@ -8,7 +8,7 @@ Mirrored surface (reference file:line):
 
 What changes underneath:
     * Linear.forward_ggml_cast_weights (ops.py:242-244) no longer materialises W through ~17 ATen kernels and
-      then calls F.linear: it hands the PACKED weight to ggufb200_linear (fused dequant + GEMV / tcgen05 GEMM).
+      then calls F.linear: it hands the PACKED weight to ggufb200_linear (fused dequant + GEMV / warpgroup-MMA GEMM).
       LoRA-patched weights, fp32 activations and CPU inputs take the two-step route (one dequant launch,
       then comfy.lora.calculate_weight / F.linear) so their semantics stay those of the reference.
     * get_weight (ops.py:166-191) dequantises with ONE kernel launch (dequant.py of this package).
@@ -143,7 +143,7 @@ def span_layout(weight, wraw):
     return out
 
 
-LORA_MAX_RANK = 64     # the LoRA k-block of the TMEM-fed kernel is one 64-wide k-block
+LORA_MAX_RANK = 64     # the LoRA k-block of the FUSED_TMEM kernel is one 64-wide k-block
 
 
 def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None):
@@ -203,7 +203,7 @@ def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None
 
 def linear_packed(x, weight, bias, dequant_dtype=None, algo=_lib.ALGO_AUTO, use_spans=False):
     """y = x @ dequant(weight).T + bias through the C ABI, weight still packed.  `algo` = _lib.ALGO_* | _lib.FLAG_*.
-    use_spans: hand the re-packed span-major copy of the weight (built once, cached on the tensor) to the TMEM-fed kernel.
+    use_spans: hand the re-packed span-major copy of the weight (built once, cached on the tensor) to the FUSED_TMEM kernel.
 
     x: CUDA fp16/bf16 [..., K]; weight: CUDA GGMLTensor (quantised type); bias: None or a CUDA tensor
     (fp32 / fp16 / bf16, rounded to x.dtype inside the kernel exactly like ops.py:205-207 does)."""
@@ -217,7 +217,7 @@ def linear_packed(x, weight, bias, dequant_dtype=None, algo=_lib.ALGO_AUTO, use_
 
 
 def linear_dense(x, weight, bias=None):
-    """y = x @ weight.T + bias on the tcgen05 GEMM with an already dense fp16/bf16 weight (ggufb200_gemm)."""
+    """y = x @ weight.T + bias on the tensor-core GEMM with an already dense fp16/bf16 weight (ggufb200_gemm)."""
     N, K = weight.shape
     x2 = x.reshape(-1, K)
     if x2.stride(-1) != 1 or (x2.stride(0) % 8) != 0 or (x2.data_ptr() % 16) != 0:
@@ -401,13 +401,13 @@ class GGMLOps(comfy_ops.manual_cast):
         # Numerics contract of the packed-weight Linear (DESIGN.md section 3, include/ggufb200.h GGUFB200_FLAG_EXACT_W):
         #   "exact"  (default) the weight operand of every route is bit-identical to the reference's
         #            `dequantize_tensor(...).to(dtype)`; only the fp32 summation order differs (<= 1e-3, measured <= 3e-4)
-        #   "fast"   the TMEM-fed kernel runs its fused-multiply-add producers (Q4_K / Q5_K: one rounding instead of two per
+        #   "fast"   the FUSED_TMEM kernel runs its fused-multiply-add producers (Q4_K / Q5_K: one rounding instead of two per
         #            element; 1e-3 for fp16 activations, 8e-3 for bf16) -- only pays off where the producers, not the tensor
         #            pipe, bound the kernel (small M)
         linear_numerics = "exact"
         # Weights whose canonical rows the TMA engine cannot stage (Q2_K / Q3_K / Q6_K / IQ4_XS, Q8_0 at K = 2432 ...) get a
         # re-packed span-major shadow copy on first use (one extra copy of the packed bytes in HBM, csrc/repack.cu) so that
-        # they too run on the TMEM-fed kernel; False keeps them on the round-1 routes (smem-fed fused / dequant + dense GEMM).
+        # they too run on the FUSED_TMEM kernel; False keeps them on the round-1 routes (smem-fed fused / dequant + dense GEMM).
         repack_spans = True
 
         def _fused_ok(self, input):
@@ -436,12 +436,7 @@ class GGMLOps(comfy_ops.manual_cast):
 
         # LoRA inside the fused kernel (csrc/gemm4.cu: one extra k-block, SURVEY 8f rank 1): U = scale * up (fp16 [N, 64]) and
         # down (act dtype [64, K]), zero padded to rank 64 and cached per patch set; per forward only T = x * down^T
-        # ([M, 64], this package's dense tcgen05 GEMM) is computed before the fused call.
-        # (Round 2 shipped this route switched off for a few hours: with several patched forwards queued back to back it hung
-        # intermittently.  Cause: the LoRA k-block shifts the next item's first k-block index off a multiple of 4, and the
-        # producers took their quarter of a span from the item-local index, so a second group became the next writer of an A
-        # stage and could pass the empty-stage parity wait on a phase two uses old.  csrc/gemm4.cu now keys the quarter on the
-        # GLOBAL k-block index -- one writer group per stage, as without LoRA.  Evidence: profiles/r02_lora_in_kernel_*.log.)
+        # ([M, 64], this package's dense tensor-core GEMM) is computed before the fused call.
         # False -> the unpatched fused kernel plus two library GEMMs of rank sum(r) (`_add_lora`).
         lora_in_kernel = True
 
@@ -508,7 +503,7 @@ class GGMLOps(comfy_ops.manual_cast):
                     exact = (_lib.FLAG_EXACT_W if self.linear_numerics != "fast" else 0) | _lib.FLAG_W_STABLE
                     algo |= exact
                     if (self.repack_spans and resident and math == _F16_CODE and N % 8 == 0 and qtype != _Q.BF16
-                            and needs_span_layout(qtype, K) and (M > GEMV_MAX_M or N * K >= (40 << 20))):
+                            and needs_span_layout(qtype, K) and M > GEMV_MAX_M):
                         spans = span_layout(w, wraw)                   # cached on the tensor after the first forward
                         algo = _lib.ALGO_FUSED_TMEM | exact
                     lora = None

@@ -1,5 +1,5 @@
 /*
- * ggufb200.h -- C ABI of libggufb200.so: B200 (sm_100a) GGUF block dequant and the
+ * ggufb200.h -- C ABI of libggufb200.so: H100 (sm_90a) GGUF block dequant and the
  * Linear that consumes the dequantised weight.
  *
  * This is the drop-in boundary for the hot path of city96/ComfyUI-GGUF.  The
@@ -14,7 +14,7 @@
  *   - all calls are asynchronous on `stream` and re-entrant; routing depends only on the arguments of the call
  *     (the library keeps no mutable routing state; ggufb200_set_tuning() is a benchmark-only switch that is refused
  *     unless the process opted in with GGUFB200_ALLOW_TUNING=1)
- *   - the device code is sm_100a only: calls that would launch a kernel return GGUFB200_E_DEVICE on any other GPU
+ *   - the device code is sm_90a only: calls that would launch a kernel return GGUFB200_E_DEVICE on any other GPU
  *   - return value: 0 = GGUFB200_OK, negative = error (ggufb200_strerror()); no C++
  *     exception crosses the boundary
  *   - ggml_type uses gguf-py's GGMLQuantizationType integer values
@@ -44,7 +44,7 @@ extern "C" {
 #define GGUFB200_E_CUDA (-6)      /* a CUDA call failed (cudaGetLastError preserved for the caller) */
 #define GGUFB200_E_WORKSPACE (-7) /* workspace smaller than ggufb200_linear_workspace() */
 #define GGUFB200_E_UNSUPPORTED (-8) /* op / dtype combination not implemented for this type */
-#define GGUFB200_E_DEVICE (-9)    /* current device is not sm_100 */
+#define GGUFB200_E_DEVICE (-9)    /* current device is not sm_90 */
 
 /* dtype codes */
 #define GGUFB200_F16 0
@@ -55,14 +55,14 @@ extern "C" {
 #define GGUFB200_OP_DEQUANT 0
 #define GGUFB200_OP_LINEAR 1
 #define GGUFB200_OP_ROWS 2
-#define GGUFB200_OP_LINEAR_MMA 3 /* large-M tcgen05 path (fused or dequant+GEMM) available for this type */
+#define GGUFB200_OP_LINEAR_MMA 3 /* large-M tensor-core path (fused or dequant+GEMM) available for this type */
 
 /* algorithm selector for ggufb200_linear(): one GGUFB200_ALGO_* value, optionally OR-ed with GGUFB200_FLAG_* bits */
 #define GGUFB200_ALGO_AUTO 0
 #define GGUFB200_ALGO_GEMV 1        /* M <= 8: fused dequant + mma.sync dot products, W bit-identical to the reference */
-#define GGUFB200_ALGO_FUSED_MMA 2   /* fused dequant -> shared memory -> tcgen05.mma (W bit-identical to the reference) */
-#define GGUFB200_ALGO_DEQUANT_MMA 3 /* dequant into the caller's workspace, then the tcgen05 GEMM on it (W bit-identical) */
-#define GGUFB200_ALGO_FUSED_TMEM 4  /* fused dequant -> TENSOR MEMORY -> tcgen05.mma, any M (persistent; what AUTO picks for M > 8) */
+#define GGUFB200_ALGO_FUSED_MMA 2   /* fused dequant -> shared memory -> wgmma (W bit-identical to the reference) */
+#define GGUFB200_ALGO_DEQUANT_MMA 3 /* dequant into the caller's workspace, then the wgmma GEMM on it (W bit-identical) */
+#define GGUFB200_ALGO_FUSED_TMEM 4  /* fused dequant -> shared memory -> wgmma with token tiles sized to M, any M (what AUTO picks for M > 8) */
 #define GGUFB200_ALGO_GEMV_FAST 5   /* M <= 8, Q4_K / Q5_K: integer patterns on mma.sync, sub-block scales applied to the partial sums
                                        (W is never formed or rounded: the `fast` contract; AUTO picks it only without EXACT_W) */
 #define GGUFB200_ALGO_MASK 0xFF
@@ -77,10 +77,10 @@ extern "C" {
  *              activation dtype.  Result as close to the exact product as the reference's, within 1e-3 (fp16) / 8e-3
  *              (bf16, = the same bound in bf16 ulps) of the reference's.
  *   GENERIC    FUSED_TMEM: functor producers that follow the reference's rounding sequence op for op (every format; also exact)
- *   TILE384    FUSED_TMEM: force 384-token items (both accumulator slots per dequantised tile, epilogue not overlapped)
- *   TILE192    FUSED_TMEM: force 192-token items (accumulator slots alternate between items); default: a cost model picks
+ *   TILE384    FUSED_TMEM: force 384-token items (two 192-token CTAs per 128 features)
+ *   TILE192    FUSED_TMEM: force 192-token items; default: a cost model picks
  *   NOSPLIT    FUSED_MMA / FUSED_TMEM: never cut K into ranges
- *   UNSTAGED   FUSED_MMA: producers read packed rows from global memory instead of TMA-staged shared memory */
+ *   UNSTAGED   accepted for compatibility, no effect: FUSED_MMA producers always read the packed rows from global memory */
 #define GGUFB200_FLAG_EXACT_W 0x100
 #define GGUFB200_FLAG_GENERIC 0x200
 #define GGUFB200_FLAG_TILE384 0x400
@@ -156,7 +156,7 @@ int ggufb200_dequant_rows(int ggml_type, const void *packed, int64_t n_table_row
  *   bias        NULL or N values of bias_dtype (0/1/2)
  *   workspace   scratch of at least ggufb200_linear_workspace() bytes (may be NULL if that is 0).  A W_packed that is
  *               not 16-byte aligned is always served by GGUFB200_ALGO_DEQUANT_MMA and needs that algo's workspace.
- *               GGUFB200_ALGO_FUSED_MMA with few output tiles (short M) cuts K into S ranges across SM pairs and keeps
+ *               GGUFB200_ALGO_FUSED_MMA with few output tiles (short M) cuts K into S ranges across SMs and keeps
  *               the fp32 partial results in the workspace (S*M*N*4 bytes, summed in a fixed order: reproducible);
  *               with less room it uses fewer ranges, with none it runs unsplit; GGUFB200_ALGO_FUSED_TMEM likewise.
  *               ggufb200_linear_workspace() assumes math_dtype == fp16 (the reference default);
@@ -175,13 +175,13 @@ int ggufb200_linear(int ggml_type, const void *W_packed, int64_t N, int64_t K, c
 
 /*
  * Span-major shadow layout (SURVEY 8f rank 3, "one-time GPU repack").  The canonical GGUF rows (loader.py:96-120) can be
- * staged by the TMA engine only when a row's 256-wide K-span and the row stride are multiples of 16 bytes; Q2_K / Q3_K /
+ * read by the FUSED_TMEM producers only when a row's 256-wide K-span and the row stride are multiples of 16 bytes; Q2_K / Q3_K /
  * Q6_K / IQ4_XS blocks (84 / 110 / 210 / 136 bytes) and e.g. Q8_0 rows of 2432 elements (2584 bytes) are not.
  * ggufb200_repack() writes a copy out[span][row padded to 256][pitch] (pitch = span bytes padded to a multiple of 16, zero
- * filled) that GGUFB200_ALGO_FUSED_TMEM stages with one bulk copy per tile for EVERY block format and every K.  The
+ * filled) that GGUFB200_ALGO_FUSED_TMEM reads with 16-byte loads for EVERY block format and every K.  The
  * canonical bytes are not modified (GGMLTensor / state_dict semantics are the reference's); the copy is a cache owned by
  * the caller: ggufb200_repack_bytes() bytes, 16-byte aligned, valid as long as the caller keeps it.
- * ggufb200_linear_spans() = ggufb200_linear() with that copy at hand: AUTO then takes the TMEM-fed kernel for every format
+ * ggufb200_linear_spans() = ggufb200_linear() with that copy at hand: AUTO then takes the FUSED_TMEM kernel for every format
  * (W_packed is still required: the reference-exact routes and EXACT_W read the canonical bytes).
  */
 size_t ggufb200_repack_bytes(int ggml_type, int64_t N, int64_t K);
@@ -195,12 +195,10 @@ int ggufb200_linear_spans(int ggml_type, const void *W_packed, const void *W_spa
  * per-forward dequant + comfy.lora.calculate_weight + F.linear of ops.py:171-190 / nodes.py:43-47 for plain LoRA patches):
  *     Y = X * dequant(W)^T + T * U^T (+ bias),   T = X * down^T  [M, 64] act_dtype (row stride ldt, zero padded beyond the
  *     total rank R <= 64),   U = scale * up  [N, 64] fp16, contiguous, zero padded.
- * The update is one extra 64-wide k-block of GGUFB200_ALGO_FUSED_TMEM (U rows go to tensor memory like a dequantised
- * span, the T tile is TMA-fed like an activation tile): no second pass over Y, no extra GEMM launch for the up-projection.
+ * The update is one extra 64-wide k-block of GGUFB200_ALGO_FUSED_TMEM (U rows take the place of a dequantised weight tile,
+ * the T tile is TMA-fed like an activation tile): no second pass over Y, no extra GEMM launch for the up-projection.
  * algo must resolve to GGUFB200_ALGO_FUSED_TMEM (AUTO without EXACT_W on a weight that route supports, or explicit),
  * otherwise GGUFB200_E_UNSUPPORTED.  W_spans may be NULL.  fp16 dequant math.
- * (Round 2 fixed an intermittent hang of this entry point under many unsynchronised back-to-back calls: two producer groups
- * could become writers of one A stage after the LoRA k-block; profiles/r02_lora_in_kernel_hang_and_fix.log.)
  */
 int ggufb200_linear_lora(int ggml_type, const void *W_packed, const void *W_spans, int64_t N, int64_t K, const void *X, int64_t M,
                          int64_t ldx, int act_dtype, const void *bias, int bias_dtype, const void *T, int64_t ldt, const void *U,
@@ -215,10 +213,10 @@ int ggufb200_gemm(const void *W, int64_t N, int64_t K, int64_t ldw, const void *
                   int act_dtype, const void *bias, int bias_dtype, void *Y, int64_t ldy, void *stream);
 
 /* Diagnostics: the tiling a fused kernel uses for this problem when given `workspace_bytes` of scratch.
- * algo = GGUFB200_ALGO_FUSED_MMA (| flags): activation rows per SM-pair tile (256 or 512), number of K ranges (1 = unsplit),
- *   64-wide k-blocks per range (the last range may be shorter, never empty), CTAs launched.
+ * algo = GGUFB200_ALGO_FUSED_MMA (| flags): activation rows per tile (128), number of K ranges (1 = unsplit),
+ *   64-wide k-blocks per range (the last range may be shorter, never empty), CTAs launched (one per 128 x 256 tile and range).
  * algo = GGUFB200_ALGO_FUSED_TMEM (| flags): tokens per item (32 / 128 / 192 / 384), number of K ranges, k-blocks per range,
- *   number of work items (persistent grid = min(items, SM pairs) clusters).
+ *   number of work items (each served by 2 CTAs of 128 features per 192 / 128 / 32 tokens).
  * Pure host arithmetic, no GPU needed. */
 int ggufb200_linear_plan(int ggml_type, int64_t M, int64_t N, int64_t K, size_t workspace_bytes, int algo, int *tile_rows, int *k_ranges,
                          int *kblocks_per_range, int *ctas);

@@ -1,7 +1,7 @@
 """The reference's torch-GPU execution path, restated for A/B timing -- TEST / BENCH INFRASTRUCTURE ONLY.
 
-/root/reference does not exist on the GPU box, so the "reference torch-GPU path" that BASELINE.json asks the
-fused kernels to beat is re-expressed here as the same chain of unfused ATen ops the reference issues per
+The reference is a ComfyUI custom-node directory that is not installed next to this package, so the "reference
+torch-GPU path" that BASELINE.json asks the fused kernels to beat is re-expressed here as the same chain of unfused ATen ops the reference issues per
 Linear call (dequant.py:30-44 -> dequantize_blocks_* -> `.to(dtype)` -> F.linear, ops.py:242-244), including
 its per-call creation of the small shift tensors on the device.  tests/test_torch_chain.py pins this file
 against the unmodified reference (bit-equal outputs AND the same number of materialising ATen kernels) in the

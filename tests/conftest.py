@@ -10,16 +10,16 @@ for p in (ROOT, os.path.join(ROOT, "tests", "fake_comfy")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90) GPU")
 
 
 def pytest_collection_modifyitems(config, items):
-    """`gpu` tests need a B200: on any other box they are reported as skipped instead of failing in torch.cuda init."""
+    """`gpu` tests need an H100: on any other machine they are reported as skipped instead of failing in torch.cuda init."""
     import torch
-    ok = torch.cuda.is_available() and torch.cuda.get_device_capability(0) == (10, 0)
+    ok = torch.cuda.is_available() and torch.cuda.get_device_capability(0) == (9, 0)
     if ok:
         return
-    why = pytest.mark.skip(reason="needs a B200 (sm_100) GPU")
+    why = pytest.mark.skip(reason="needs an H100 (sm_90) GPU")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(why)
@@ -29,8 +29,8 @@ def pytest_collection_modifyitems(config, items):
 def pkg():
     import __graft_entry__ as ge
     ge.load_package()
-    # A/B runs of kernel variants (tools/gpu_*.sh only): GGUFB200_ALLOW_TUNING=1 GGUFB200_TEST_TUNING="key=value[,key=value]"
-    # runs the suite with bench-only launch knobs set.  Never set in the driver's runs.
+    # A/B runs of kernel variants: GGUFB200_ALLOW_TUNING=1 GGUFB200_TEST_TUNING="key=value[,key=value]" runs the suite with
+    # bench-only launch knobs set.
     for kv in filter(None, os.environ.get("GGUFB200_TEST_TUNING", "").split(",")):
         k, v = kv.split("=")
         assert ge._sub("_lib").lib().ggufb200_set_tuning(int(k), int(v)) == 0

@@ -11,6 +11,12 @@ What is produced (all under tests/golden/):
   linear_<QTYPE>_<act>.npz   x / packed W / F32 bias and the output of the
                         reference `ops.py::GGMLOps.Linear.forward` (run on CPU
                         through tests/fake_comfy)
+  reference_surface.json   public function / class names of the reference's
+                        dequant.py and ops.py
+  torch_chain.json      the reference's `dequantize(raw, qtype, shape, dtype)` on
+                        96 seeded blocks per (qtype, math dtype): dtype, SHA-256 of
+                        the result's bytes, and the number of materialising ATen
+                        kernels it ran
 
 The reference is imported by path and never copied: dequant.py via importlib,
 ops.py through a throw-away package directory of symlinks in $TMPDIR.
@@ -135,8 +141,46 @@ def make_linear(refops):
         print("wrote linear", qt.name)
 
 
+def make_surface():
+    import ast
+    import json
+
+    def public(path):
+        tree = ast.parse(open(path).read())
+        return sorted(n.name for n in tree.body if isinstance(n, (ast.FunctionDef, ast.ClassDef)) and not n.name.startswith("_"))
+    with open(os.path.join(HERE, "reference_surface.json"), "w") as f:
+        json.dump({m: public(os.path.join(REF, m)) for m in ("dequant.py", "ops.py")}, f, indent=1)
+        f.write("\n")
+
+
+CHAIN_QTYPES = [T.Q8_0, T.Q4_0, T.Q4_K, T.Q5_K, T.Q6_K, T.BF16]
+CHAIN_MATH = {"none": None, "float32": torch.float32, "bfloat16": torch.bfloat16}
+
+
+def make_torch_chain(ref):
+    import hashlib
+    import json
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_torch_chain import Count      # the same kernel counter the test applies to oracle/torch_chain.py
+    out = {}
+    for qt in CHAIN_QTYPES:
+        bs, _ts = gguf.GGML_QUANT_SIZES[qt]
+        raw = torch.from_numpy(oracle.random_blocks(int(qt), 96, seed=1)).reshape(-1)
+        for name, md in CHAIN_MATH.items():
+            with Count() as c:
+                y = ref.dequantize(raw, qt, (96 * bs,), dtype=md)
+            raw_bytes = y.contiguous().view(torch.uint8).numpy()
+            out[f"{qt.name}_{name}"] = {"dtype": str(y.dtype), "kernels": c.n, "nbytes": int(raw_bytes.size),
+                                        "sha256": hashlib.sha256(raw_bytes.tobytes()).hexdigest()}
+    with open(os.path.join(HERE, "torch_chain.json"), "w") as f:
+        json.dump(out, f, indent=1, sort_keys=True)
+        f.write("\n")
+
+
 if __name__ == "__main__":
     torch.manual_seed(0)
     make_dequant(load_ref_dequant())
     make_linear(load_ref_ops())
+    make_surface()
+    make_torch_chain(load_ref_dequant())
     print("total bytes:", sum(os.path.getsize(os.path.join(HERE, f)) for f in os.listdir(HERE) if f.endswith(".npz")))

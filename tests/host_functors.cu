@@ -69,7 +69,7 @@ template <class Q, int ACT> int run_fast16(const uint8_t *blocks, long long n_bl
     }
 }
 
-// W producers of the TMEM-fed fused kernel (produce.cuh): spans of `span_bytes` per row, 16-byte aligned, rows of
+// W producers of the fused kernels (produce.cuh): spans of `span_bytes` per row, 16-byte aligned, rows of
 // 256 elements; out: fp16 bit patterns, n_spans * 256 elements
 template <class Q, int PROD> int run_produce(const uint8_t *spans, long long n_spans, int pitch, uint16_t *out)
 {
@@ -130,34 +130,5 @@ int hostf_produce(int type, const uint8_t *spans, long long n_spans, int pitch, 
 void hostf_k_scale_min(const uint8_t *s12, int j, int *sc, int *mn) { k_scale_min(s12, j, *sc, *mn); }
 uint32_t hostf_iq4_lookup4(uint32_t idx4) { return iq4_lookup4(idx4); }
 uint32_t hostf_prmt(uint32_t a, uint32_t b, uint32_t sel) { return prmt(a, b, sel); }
-
-// The producer bookkeeping of gemm4.cu's dequant groups over a sequence of items (nspans[i] spans, lora[i] = 1: one extra LoRA
-// k-block), with the product's own group -> quarter mapping (produce.cuh): writer[it] = the group that writes global k-block
-// `it` (-1: nobody, -2: written twice), quarter[it] = which quarter of its span that k-block is (4: the LoRA k-block).
-// legacy != 0 reproduces round 2's first mapping (quarter = group, LoRA by group 0) for the regression test.
-int hostf_g4_schedule(const int *nspans, const int *lora, int n_items, int legacy, int *writer, int *quarter, int n_slots)
-{
-    for (int i = 0; i < n_slots; ++i) writer[i] = -1, quarter[i] = -1;
-    for (int g = 0; g < 4; ++g) {
-        int it0 = 0;
-        for (int item = 0; item < n_items; ++item) {
-            const int qr = legacy ? g : g4_group_quarter(g, it0);
-            for (int i = 0; i < nspans[item]; ++i) {
-                const int it = it0 + 4 * i + qr;
-                if (it >= n_slots) return -1;
-                writer[it] = writer[it] == -1 ? g : -2;
-                quarter[it] = qr;
-            }
-            if (lora[item] && g == (legacy ? 0 : g4_lora_group(it0, nspans[item]))) {
-                const int it = it0 + 4 * nspans[item];
-                if (it >= n_slots) return -1;
-                writer[it] = writer[it] == -1 ? g : -2;
-                quarter[it] = 4;
-            }
-            it0 += 4 * nspans[item] + (lora[item] ? 1 : 0);
-        }
-    }
-    return 0;
-}
 
 }  // extern "C"

@@ -99,14 +99,14 @@ def test_workspace_contract_follows_the_route(pkg):
     assert ws(q4k, 4608, 3072, 3072, 1, A.ALGO_FUSED_MMA) == 0                        # enough tiles: unsplit
     assert ws(q4k, 64, 512, 4096, 1, A.ALGO_FUSED_MMA) == 16 * 64 * 512 * 4           # split-K: 16 slices
     assert ws(q4k, 64, 512, 4096, 1, A.ALGO_FUSED_MMA | A.FLAG_NOSPLIT) == 0
-    assert ws(q4k, 512, 3072, 12288, 1, A.ALGO_FUSED_MMA) == 6 * 512 * 3072 * 4       # 12 tiles of 512x256 -> 6 ranges
-    # AUTO: the TMEM-fed fused kernel for every M > 8 and for M <= 8 on large weights (K ranges only when that beats idle SM
-    # pairs by the cost model); EXACT_W only changes its producers, never the route or the workspace
+    assert ws(q4k, 512, 3072, 12288, 1, A.ALGO_FUSED_MMA) == 2 * 512 * 3072 * 4       # 48 tiles of 128x256 -> 2 ranges
+    # AUTO: the FUSED_TMEM kernel for every M > 8 (K ranges only when that beats idle
+    # SMs by the cost model); EXACT_W only changes its producers, never the route or the workspace
     for flags in (0, A.FLAG_EXACT_W):
         auto = A.ALGO_AUTO | flags
         assert ws(q4k, 4608, 3072, 3072, 1, auto) == 0
         assert ws(q4k, 4, 3072, 3072, 1, auto) == 0                                   # small weight at M <= 8: mma.sync GEMV
-        assert ws(q4k, 4, 18432, 3072, 1, auto) == 0                                  # large weight at M <= 8: TMEM kernel, 72 items, unsplit
+        assert ws(q4k, 4, 18432, 3072, 1, auto) == 0                                  # large weight at M <= 8: a GEMV as well
         assert ws(q4k, 64, 512, 4096, 1, auto) == ws(q4k, 64, 512, 4096, 1, A.ALGO_FUSED_TMEM) > 0
         assert ws(q4k, 64, 512, 4096, 1, auto) % (64 * 512 * 4) == 0
         assert ws(q4k, 64, 512, 4096, 1, auto | A.FLAG_NOSPLIT) == 0
@@ -116,7 +116,7 @@ def test_workspace_contract_follows_the_route(pkg):
     assert wx(q4k, 64, 512, 4096, 1, 2, A.ALGO_AUTO) == 512 * 4096 * 2
     assert wx(q4k, 4, 3072, 3072, 1, 2, A.ALGO_AUTO) == 0
     assert wx(q4k, 64, 512, 4096, 1, 0, A.ALGO_AUTO) == ws(q4k, 64, 512, 4096, 1, A.ALGO_AUTO)
-    # formats / shapes the TMEM route cannot stage from the canonical rows (no span-major copy at hand) fall back to round 1's routes
+    # formats / shapes the FUSED_TMEM route cannot read from the canonical rows (no span-major copy at hand) fall back to round 1's routes
     assert ws(int(Q.Q6_K), 4608, 3072, 3072, 1, A.ALGO_AUTO) == 3072 * 3072 * 2       # 210-byte blocks
     assert ws(int(Q.Q8_0), 4608, 7296, 2432, 1, A.ALGO_AUTO) == 7296 * 2432 * 2       # 2584-byte rows
     # row gather: K must be a multiple of the block size
@@ -145,7 +145,7 @@ def test_span_layout_geometry_without_gpu(pkg):
     assert L.ggufb200_repack(int(Q.BF16), p16, 8, 8, p16, None) == -1
     assert L.ggufb200_repack(int(Q.Q4_K), None, 8, 256, p16, None) == -5
     assert L.ggufb200_repack(int(Q.Q4_K), p16, 8, 256, p16 + 4, None) == -3
-    # the LoRA entry point validates like ggufb200_linear and needs the TMEM route
+    # the LoRA entry point validates like ggufb200_linear and needs the FUSED_TMEM route
     x = p16
     assert L.ggufb200_linear_lora(int(Q.Q4_K), p16, None, 8, 256, x, 4, 256, 1, None, 0, x, 64, x, x, 8, None, 0,
                                   pkg.lib.ALGO_GEMV, None) == -8

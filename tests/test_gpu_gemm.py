@@ -1,5 +1,5 @@
 """GPU parity tests of the tensor-core Linear kernels: dense TMA-fed GEMM (csrc/gemm3.cu), the shared-memory-fed fused
-kernel (csrc/gemm2.cu, reference-exact W) and the TMEM-fed fused kernel (csrc/gemm4.cu, the AUTO default).
+kernel (csrc/gemm2.cu, reference-exact W) and the FUSED_TMEM kernel (csrc/gemm4.cu, the AUTO default).
 
 Reference: fp32-accumulated x @ W^T (+bias) rounded to the activation dtype, where W is the bit-exact dequantised weight
 (validated separately against the reference's golden outputs).
@@ -167,7 +167,7 @@ def test_fused_gemm_flux_shapes_q4k(pkg, M, N, K):
         assert err_ours <= 1.05 * err_ref, (algo, err_ours, err_ref)
 
 
-# ---------------------------------------------------------------- TMEM-fed fused kernel (csrc/gemm4.cu)
+# ---------------------------------------------------------------- FUSED_TMEM kernel (csrc/gemm4.cu)
 PRODUCERS = {"fast": 0, "generic": 0x200, "exact": 0x100}      # default / GGUFB200_FLAG_GENERIC / GGUFB200_FLAG_EXACT_W
 
 
@@ -212,9 +212,9 @@ def test_tmem_fused_shapes(pkg, M, N, K, tile384):
 
 
 def test_tmem_fused_many_items_per_pair(pkg):
-    """More items than SM pairs: every pair walks several (feature tile, token tile) items -- exercises the accumulator
-    double buffering and the ring parities across item boundaries."""
-    M, N, K = 1536, 8192, 512          # 32 feature tiles x 8 token tiles = 256 items on 74 pairs
+    """More CTAs than SMs: several waves of (feature tile, token tile) CTAs, with 192- and 384-token items -- exercises the
+    tile decode of the grid and the ring parities over long K loops."""
+    M, N, K = 1536, 8192, 512          # 32 feature tiles x 8 token tiles = 256 items, 512 CTAs on 132 SMs
     _raw, w = _weight(pkg, Q.Q4_K, N, K, seed=77)
     x = torch.randn(M, K, device=DEV, dtype=torch.float16)
     W = pkg.dequant.dequantize_tensor(w, torch.float16)
@@ -273,7 +273,7 @@ def test_repack_layout_is_a_pure_byte_permutation(pkg, qt, N, K):
 @pytest.mark.parametrize("qt", BLOCK_TYPES, ids=lambda q: q.name)
 @pytest.mark.parametrize("dt", [torch.bfloat16, torch.float16], ids=["bf16", "f16"])
 def test_tmem_fused_from_span_layout_all_types(pkg, qt, dt, producers):
-    """Every block format -- including the ones no tensor map can stage (Q2_K / Q3_K / Q6_K / IQ4_XS) -- on the TMEM-fed kernel."""
+    """Every block format -- including the ones no tensor map can stage (Q2_K / Q3_K / Q6_K / IQ4_XS) -- on the FUSED_TMEM kernel."""
     M, N, K = 300, 264, 1024
     _raw, w = _weight(pkg, qt, N, K, seed=int(qt) + 5)
     x = torch.randn(M, K, device=DEV, dtype=dt)
@@ -293,7 +293,7 @@ def test_tmem_fused_from_span_layout_all_types(pkg, qt, dt, producers):
 
 @pytest.mark.parametrize("M", [2, 700])
 def test_sd35_shape_q8_0_rows_run_on_the_tmem_kernel_through_the_layer(pkg, M):
-    """SD3.5-large hidden size 2432: 2584-byte Q8_0 rows.  The layer builds the span-major copy on first use and the TMEM-fed
+    """SD3.5-large hidden size 2432: 2584-byte Q8_0 rows.  The layer builds the span-major copy on first use and the FUSED_TMEM
     kernel serves it (K = 2432 is not a multiple of 256: the last span is half empty); at M = 2 this 17.7 M-element weight stays on
     the mma.sync GEMV."""
     N, K = 7296, 2432
@@ -302,7 +302,7 @@ def test_sd35_shape_q8_0_rows_run_on_the_tmem_kernel_through_the_layer(pkg, M):
     lin.load_state_dict({"weight": w})
     x = torch.randn(M, K, device=DEV, dtype=torch.float16)
     y = lin(x)
-    # the span-major copy is built for the TMEM-fed kernel only: M > 8, or M <= 8 on a weight large enough for that kernel to win
+    # the span-major copy is built for the FUSED_TMEM kernel only: M > 8, or M <= 8 on a weight large enough for that kernel to win
     assert ("_gg_spans" in lin.weight.__dict__) == (M > 8)
     W = pkg.dequant.dequantize_tensor(w, torch.float16)
     assert rel_fro(y.float().cpu().numpy(), _ref(x, W, None).float().cpu().numpy()) <= TOL

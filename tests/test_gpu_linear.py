@@ -3,7 +3,7 @@
 Tolerance (written here, from BASELINE.json north_star): ||y - y_ref||_F / ||y_ref||_F <= 1e-3 for fp16/bf16 Linear
 outputs; y_ref is the unmodified reference's GGMLOps.Linear output (golden files) or the CPU oracle.
 Every layer-level test runs under both numerics contracts of GGMLOps.Linear (`linear_numerics`): "exact" (the default: weight
-operand bit-identical to the reference's: 1e-3 in every dtype) and "fast" (fused-multiply-add producers on the TMEM-fed
+operand bit-identical to the reference's: 1e-3 in every dtype) and "fast" (fused-multiply-add producers on the FUSED_TMEM
 kernel: 1e-3 for fp16 activations, 8e-3 = the same bound in bf16 ulps for bf16 activations -- see tests/test_gpu_gemm.py and
 DESIGN.md section 3)."""
 import os
@@ -154,8 +154,8 @@ def test_lora_on_packed_weight_runs_as_side_gemms(pkg, M, N, K, dtype, n_loras, 
     lin, x, ref, ideal = _lora_case(pkg, M, N, K, dtype, n_loras)
     assert lin._lora_terms(x.device), "LoRA-only patch list must be recognised"
     if numerics == "fast":
-        # default route (GGMLOps.Linear.lora_in_kernel = True): base product AND the rank-r update inside the TMEM-fed kernel (one
-        # extra k-block: U = scale*up rows in tensor memory, T = x*down^T TMA-fed); same budget against the reference arithmetic,
+        # default route (GGMLOps.Linear.lora_in_kernel = True): base product AND the rank-r update inside the FUSED_TMEM kernel (one
+        # extra k-block: U = scale*up rows as the weight tile, T = x*down^T TMA-fed); same budget against the reference arithmetic,
         # and within bf16 / fp16 output rounding of the side-GEMM formulation
         y_in = lin(x)
         lin.lora_in_kernel = False

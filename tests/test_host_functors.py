@@ -31,7 +31,7 @@ def hostf():
     deps = [SRC, os.path.join(CSRC, "blocks.cuh"), os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "produce.cuh")]
     if not os.path.exists(OUT) or any(os.path.getmtime(d) > os.path.getmtime(OUT) for d in deps):
         os.makedirs(os.path.dirname(OUT), exist_ok=True)
-        subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-std=c++17", "--expt-relaxed-constexpr",
+        subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-std=c++17", "--expt-relaxed-constexpr",
                         "-Xcompiler", "-fPIC,-ffp-contract=off", "-shared", "-o", OUT, SRC], check=True)
     L = ctypes.CDLL(OUT)
     L.hostf_dequant.argtypes = [ctypes.c_int, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_void_p, ctypes.c_int, ctypes.c_int]
@@ -169,7 +169,7 @@ def test_functors_never_read_past_the_last_block(tmp_path):
         pytest.skip("toolchain not available")
     obj, exe = str(tmp_path / "hf.o"), str(tmp_path / "asan_run")
     san = "-fsanitize=address,-fsanitize=undefined,-fno-sanitize=alignment"   # 2-byte aligned blocks are read with 16-bit loads by design
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-g", "-std=c++17", "--expt-relaxed-constexpr",
+    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-g", "-std=c++17", "--expt-relaxed-constexpr",
                         "-Xcompiler", "-fPIC,-ffp-contract=off," + san, "-c", SRC, "-o", obj], capture_output=True, text=True)
     if r.returncode != 0:
         pytest.skip("sanitizer build not available: " + r.stderr[-200:])
@@ -182,7 +182,7 @@ def test_functors_never_read_past_the_last_block(tmp_path):
     assert run.returncode == 0 and "asan run ok" in run.stdout, run.stderr[-2000:]
 
 
-# ---------------------------------------------------------------- produce.cuh: W producers of the TMEM-fed fused kernel
+# ---------------------------------------------------------------- produce.cuh: W producers of the fused kernels
 EXACT_FAST = {Q.Q8_0, Q.Q4_0, Q.Q6_K}          # hand-written producers whose float step already has a single rounding
 FMA_FAST = {Q.Q4_K, Q.Q5_K}                    # one fused multiply-add instead of multiply + subtract
 
@@ -253,7 +253,7 @@ def test_fast_producers(hostf, qt):
 @pytest.mark.parametrize("qt", sorted(EXACT_FAST | FMA_FAST, key=int), ids=lambda q: q.name)
 @pytest.mark.parametrize("wild", [False, True], ids=["trained-like", "raw-bytes"])
 def test_hand_written_producers_with_the_reference_sequence_are_bit_exact(hostf, qt, wild):
-    """FastProducer<Q, FMA = false> (GGUFB200_FLAG_EXACT_W on the TMEM route): the weight is the reference's, bit for bit."""
+    """FastProducer<Q, FMA = false> (GGUFB200_FLAG_EXACT_W on the FUSED_TMEM route): the weight is the reference's, bit for bit."""
     n = 1500
     bs, ts = oracle.type_info(int(qt))
     span = 256 // bs * ts
@@ -270,35 +270,3 @@ def test_fast_request_falls_back_to_generic_for_other_formats(hostf):
     assert hostf.hostf_produce(int(Q.Q3_K), buf.ctypes.data, 8, pitch, got.ctypes.data, 1) == 0
     want = oracle.dequant(raw.reshape(-1, 110), int(Q.Q3_K), oracle.DT_F16, oracle.DT_F16)
     assert _equal_mod_nan(got, want, oracle.DT_F16)
-
-
-# ---------------------------------------------------------------- gemm4: one writer group per A stage (the LoRA hang of round 2)
-def test_g4_one_writer_group_per_a_stage(hostf):
-    """csrc/gemm4.cu keeps dequantised k-blocks in a ring of A stages (a multiple of 4) and relies on ONE producer group per
-    stage: group g must write exactly the k-blocks whose global index is == g (mod 4), whatever mix of items with and without
-    a LoRA k-block a CTA pair walks through -- otherwise a parity wait on a stage can be satisfied by a phase two uses old
-    (profiles/r02_lora_in_kernel_hang_and_fix.log).  The MMA warp consumes the k-blocks of an item in order, so the k-block
-    with item-local index j must also be quarter j % 4 of span j / 4 (and the last one of a LoRA item the LoRA k-block)."""
-    hostf.hostf_g4_schedule.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int]
-    rng = np.random.default_rng(5)
-    for trial in range(200):
-        n_items = int(rng.integers(1, 9))
-        nspans = rng.integers(1, 14, size=n_items).astype(np.int32)
-        lora = (rng.random(n_items) < (0.0 if trial % 4 == 0 else 0.6)).astype(np.int32)
-        total = int((4 * nspans + lora).sum())
-        writer = np.empty(total, dtype=np.int32)
-        quarter = np.empty(total, dtype=np.int32)
-        assert hostf.hostf_g4_schedule(nspans.ctypes.data, lora.ctypes.data, n_items, 0, writer.ctypes.data, quarter.ctypes.data, total) == 0
-        assert np.array_equal(writer, np.arange(total) % 4), (nspans, lora, writer)        # every index once, by group it % 4
-        it0 = 0
-        for n, l in zip(nspans, lora):                                                       # consumption order of the MMA warp
-            want = [j % 4 for j in range(4 * n)] + ([4] if l else [])
-            assert quarter[it0:it0 + len(want)].tolist() == want
-            it0 += len(want)
-    # the first round-2 mapping (quarter = group, LoRA by group 0) breaks the ownership as soon as an item follows a LoRA item
-    nspans = np.array([3, 3], dtype=np.int32)
-    lora = np.array([1, 0], dtype=np.int32)
-    writer = np.empty(25, dtype=np.int32)
-    quarter = np.empty(25, dtype=np.int32)
-    assert hostf.hostf_g4_schedule(nspans.ctypes.data, lora.ctypes.data, 2, 1, writer.ctypes.data, quarter.ctypes.data, 25) == 0
-    assert not np.array_equal(writer, np.arange(25) % 4)

@@ -2,7 +2,7 @@
 
 A wrong plan is the kind of bug that HANGS a GPU (a K range with no k-blocks never signals its barriers), so the invariants
 are checked here on the CPU over many shapes: every K range owns whole 256-wide spans, none is empty, together they cover K
-exactly once, the slices fit the workspace, the grid fits the 74 SM pairs when K is split, and the workspace query, the plan
+exactly once, the slices fit the workspace, the grid fits one wave of the 132 SMs when K is split, and the workspace query, the plan
 and the AUTO routing agree with each other."""
 import ctypes
 
@@ -11,8 +11,8 @@ from hypothesis import given, settings, strategies as st
 
 from util import Q
 
-PAIRS = 74          # 148 SMs (sm_count() reports 148 without a device as well)
-CAP = 64 << 20
+SMS = 132           # an H100 SXM (sm_count() reports 132 without a device as well)
+CAP = 24 << 20
 
 
 FUSED_MMA, FUSED_TMEM, NOSPLIT, TILE384, TILE192 = 2, 4, 0x800, 0x400, 0x2000
@@ -27,29 +27,28 @@ def _plan(L, qt, M, N, K, ws, algo=FUSED_MMA):
 def _check(L, M, N, K, ws):
     rc, (rows, ranges, kb, ctas) = _plan(L, Q.Q4_K, M, N, K, ws)
     assert rc == 0
-    assert rows in (256, 512) and ranges >= 1 and kb >= 1
+    assert rows == 128 and ranges >= 1 and kb >= 1
     total_kb = K // 64
     tiles = -(-M // rows) * -(-N // 256)
-    assert ctas == 2 * tiles * ranges
+    assert ctas == tiles * ranges                                # one CTA per (128 x 256 tile, K range)
     if ranges == 1:
         assert kb == total_kb
         return ranges
     assert K % 256 == 0 and kb % 4 == 0                        # whole spans per range
     assert (ranges - 1) * kb < total_kb <= ranges * kb          # no empty range, full cover
-    assert ranges <= 16 and tiles * ranges <= PAIRS             # one wave of SM pairs
+    assert ranges <= 16 and ctas <= SMS                         # one wave of CTAs
     assert ranges * M * N * 4 <= min(ws, CAP)                   # slices fit what the caller gave (and the L2 budget)
-    if M > 256:
-        assert rows == 512 or -(-M // 512) * -(-N // 256) * 2 > PAIRS
     return ranges
 
 
 def test_known_plans(pkg):
     L = pkg.lib.lib()
-    assert _plan(L, Q.Q4_K, 512, 3072, 12288, CAP) == (0, (512, 6, 32, 144))      # the ncu'd launch: 12 tiles x 6 ranges
-    assert _plan(L, Q.Q5_K, 512, 4096, 4096, CAP) == (0, (512, 4, 16, 128))        # T5 q/k/v/o
+    assert _plan(L, Q.Q4_K, 512, 3072, 12288, CAP) == (0, (128, 2, 96, 96))       # 48 tiles x 2 ranges
+    assert _plan(L, Q.Q4_K, 64, 3072, 12288, CAP) == (0, (128, 10, 20, 120))      # 12 tiles x 10 ranges
+    assert _plan(L, Q.Q5_K, 512, 4096, 4096, CAP) == (0, (128, 2, 32, 128))        # T5 q/k/v/o
     assert _plan(L, Q.Q4_K, 4608, 3072, 3072, CAP)[1][1] == 1                      # plenty of tiles: unsplit
     assert _plan(L, Q.Q4_K, 512, 3072, 12288, 0)[1][1] == 1                        # no workspace: unsplit
-    assert _plan(L, Q.Q4_K, 512, 3072, 12288, 3 * 512 * 3072 * 4)[1][1] == 3       # smaller workspace: fewer ranges
+    assert _plan(L, Q.Q4_K, 64, 3072, 12288, 3 * 64 * 3072 * 4)[1][1] == 3         # smaller workspace: fewer ranges
     assert _plan(L, Q.Q4_K, 64, 512, 4096 + 64, CAP)[1][1] == 1                    # K not a multiple of 256: unsplit
     assert _plan(L, Q.BF16, 64, 512, 4096, CAP)[0] == -8                           # no fused kernel for dense weights
     assert _plan(L, Q.Q4_K, 64, 512, 4000, CAP)[0] == -4
@@ -81,7 +80,7 @@ def test_nosplit_flag_disables_every_split(pkg):
         assert L.ggufb200_linear_workspace(int(Q.Q4_K), M, N, K, 1, FUSED_TMEM | NOSPLIT) == 0
 
 
-# ---------------------------------------------------------------- TMEM-fed kernel (csrc/gemm4.cu::g4_plan)
+# ---------------------------------------------------------------- FUSED_TMEM kernel (csrc/gemm4.cu::g4_plan)
 def _check_tmem(L, M, N, K, ws, flags=0):
     rc, (tokens, ranges, kb, items) = _plan(L, Q.Q4_K, M, N, K, ws, FUSED_TMEM | flags)
     assert rc == 0
@@ -107,10 +106,10 @@ def test_known_tmem_plans(pkg):
     L = pkg.lib.lib()
     assert _plan(L, Q.Q4_K, 4608, 12288, 3072, CAP, FUSED_TMEM | TILE192) == (0, (192, 1, 48, 48 * 24))      # Flux mlp.0: 1152 items
     assert _plan(L, Q.Q4_K, 4608, 12288, 3072, CAP, FUSED_TMEM | TILE384) == (0, (384, 1, 48, 48 * 12))
-    assert _plan(L, Q.Q4_K, 4608, 12288, 3072, CAP, FUSED_TMEM) == (0, (384, 1, 48, 48 * 12))               # the cost model's pick
-    assert _plan(L, Q.Q4_K, 512, 3072, 12288, CAP, FUSED_TMEM) == (0, (192, 2, 96, 72))                      # 36 tiles x 2 K ranges
-    assert _plan(L, Q.Q4_K, 1, 18432, 3072, CAP, FUSED_TMEM) == (0, (32, 1, 48, 72))               # modulation GEMV: one item per pair
-    assert _plan(L, Q.Q4_K, 1, 3072, 3072, CAP, FUSED_TMEM) == (0, (32, 6, 8, 72))                 # 12 feature tiles x 6 K ranges
+    assert _plan(L, Q.Q4_K, 4608, 12288, 3072, CAP, FUSED_TMEM) == (0, (192, 1, 48, 48 * 24))               # the cost model's pick
+    assert _plan(L, Q.Q4_K, 512, 3072, 12288, CAP, FUSED_TMEM) == (0, (192, 3, 64, 108))                     # 36 tiles x 3 K ranges
+    assert _plan(L, Q.Q4_K, 1, 18432, 3072, CAP, FUSED_TMEM) == (0, (32, 4, 12, 288))              # modulation GEMV shape: 72 feature tiles x 4 K ranges
+    assert _plan(L, Q.Q4_K, 1, 3072, 3072, CAP, FUSED_TMEM) == (0, (32, 4, 12, 48))                # 12 feature tiles x 4 K ranges
     assert _plan(L, Q.Q4_K, 1, 3072, 3072, 0, FUSED_TMEM)[1][1] == 1                               # no workspace: unsplit
     assert _plan(L, Q.Q5_K, 512, 4096, 4096, CAP, FUSED_TMEM) == (0, (128, 1, 64, 64))             # T5 q/k/v/o at 512 tokens
     assert _plan(L, Q.BF16, 64, 512, 4096, CAP, FUSED_TMEM)[0] == -8

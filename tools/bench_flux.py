@@ -67,8 +67,8 @@ class LinearTimer:
         return float(sum(a.elapsed_time(b) for a, b in self.pairs)), len(self.pairs)
 
 
-ROUTE_NAMES = {"exact": "fused dequant -> TMEM -> tcgen05 (gemm4, persistent), reference-sequence producers: weight operand bit-identical to the reference's",
-               "fast": "fused dequant -> TMEM -> tcgen05 (gemm4, persistent), fused-multiply-add producers; M <= 8: integer-pattern mma.sync kernel (gemv2)"}
+ROUTE_NAMES = {"exact": "fused dequant -> shared memory -> wgmma (gemm4), reference-sequence producers: weight operand bit-identical to the reference's",
+               "fast": "fused dequant -> shared memory -> wgmma (gemm4), fused-multiply-add producers; M <= 8: integer-pattern mma.sync kernel (gemv2)"}
 
 
 def run(depth=19, depth_single=38, steps=10, warmup=3, ref_steps=3, txt_tokens=512, img_tokens=4096, device="cuda:0", numerics="exact",

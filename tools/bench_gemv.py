@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """GPU-side time of the small-M fused Linear (K3): raw C-ABI launches replayed from a CUDA graph (no Python / launch
 overhead in the number), weights rotated through > L2 worth of buffers.  Routes: the integer-pattern mma.sync kernel (gemv2.cu, `fast` contract), the
-TMEM-fed fused kernel (32-token items, K ranges across SM pairs) and the reference-exact mma.sync GEMV.  Prints GB/s of packed weight read vs the
+FUSED_TMEM kernel (32-token items, K ranges across SMs) and the reference-exact mma.sync GEMV.  Prints GB/s of packed weight read vs the
 measured HBM peak."""
 import json
 import os
@@ -18,7 +18,7 @@ import oracle  # noqa: E402
 ops, lib = ge._sub("ops"), ge._sub("_lib")
 L = lib.lib()
 dev = torch.device("cuda:0")
-peak = 6574.5
+peak = 3350.0      # H100 SXM data sheet, GB/s
 try:
     peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
 except Exception:

@@ -16,7 +16,7 @@ import oracle  # noqa: E402
 lib = ge._sub("_lib")
 L = lib.lib()
 dev = torch.device("cuda:0")
-peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6574.5
+peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0   # H100 SXM data sheet
 side = torch.cuda.Stream()
 OUT = ((0, torch.float16, "f16"), (1, torch.bfloat16, "bf16"), (2, torch.float32, "f32"))
 names = sys.argv[1:] or ["Q4_0", "Q4_1", "Q5_0", "Q5_1", "Q8_0", "Q2_K", "Q3_K", "Q4_K", "Q5_K", "Q6_K", "IQ4_NL", "IQ4_XS"]

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Per-shape timing of the quantised Linear at Flux.1 shapes: TMEM-fed fused tcgen05 (tmem, tmem384, tmem_generic), smem-fed
-fused tcgen05 (fused), dequant+tcgen05 (dq_mma), K1 dequant + cuBLAS, cuBLAS on a pre-dequantised weight, the reference's
+"""Per-shape timing of the quantised Linear at Flux.1 shapes: FUSED_TMEM (tmem, tmem384, tmem_generic), FUSED_MMA with
+reference-exact producers (fused), dequant + dense GEMM (dq_mma), K1 dequant + cuBLAS, cuBLAS on a pre-dequantised weight, the reference's
 torch chain.  CUDA events, weights rotated through >L2 worth of distinct buffers.  Prints one line per (shape, route): ms,
 TFLOP/s and the relative error against fp32-accumulated x @ bf16(W)^T of the SAME weight the timed call used."""
 import argparse

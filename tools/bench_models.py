@@ -149,7 +149,7 @@ def parity(which, numerics):
         out = lp.summary()
     out.update(model=which, numerics=numerics, activation="bf16",
                budget="1e-3 (exact: weight operand bit-identical to the reference's)" if numerics == "exact" else
-                      "8e-3 (fast, bf16 = 1e-3 in fp16 ulps; the TMEM route keeps W in fp16)")
+                      "8e-3 (fast, bf16 = 1e-3 in fp16 ulps)")
     del model
     torch.cuda.empty_cache()
     return out

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (read with `ncu -i ... --page raw --csv`) into the handful of numbers profiles/ keeps."""
+"""Summarise an .ncu-rep (read with `ncu -i ... --page raw --csv`) into a handful of numbers per kernel."""
 import csv
 import io
 import subprocess

@@ -17,7 +17,7 @@ import oracle  # noqa: E402
 lib = ge._sub("_lib")
 L = lib.lib()
 dev = torch.device("cuda:0")
-peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6574.5
+peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0   # H100 SXM data sheet
 side = torch.cuda.Stream()
 for qname in (sys.argv[1:] or ["Q4_K", "Q8_0"]):
     qt = gguf.GGMLQuantizationType[qname]
