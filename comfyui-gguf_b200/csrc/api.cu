@@ -1,62 +1,23 @@
 // api.cu -- the extern "C" boundary declared in include/ggufb200.h.
-// Argument validation and route selection live here; kernels live in dequant.cu / rows.cu / gemv.cu / gemm2.cu /
-// gemm3.cu / gemm4.cu / repack.cu.  Routing is a pure function of the call's arguments (algo | flags): no process-wide
-// routing state.
+// Argument validation and route selection live here; kernels live in dequant.cu / rows.cu / gemv.cu / gemv2.cu /
+// linear_sm90.cu / repack.cu (declared in internal.h).  Routing is a pure function of the call's arguments (algo | flags):
+// no process-wide routing state.
 #include <stdlib.h>
 
 #include "blocks.cuh"
-
-namespace ggufb200 {
-extern int g_dequant_pdl;
-extern int g_gemv2_ctas;
-int dequant_dispatch(int type, const void *packed, long long n_blocks, void *out, int out_dtype, int math_dtype, cudaStream_t st, bool stable = false);
-int unpack_dispatch(int type, const void *packed, long long n_blocks, int16_t *q, int16_t *sc, int16_t *mn, cudaStream_t st);
-int rows_dispatch(int type, const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows,
-                  void *out, int out_dtype, int math_dtype, cudaStream_t st);
-int gemv_dispatch(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype,
-                  int math_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st);
-int gemm2_fused_dispatch(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype,
-                         int math_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes, int flags,
-                         cudaStream_t st);
-int gemm2_fused_splits(long long M, long long N, long long K);
-void gemm2_fused_plan_info(long long M, long long N, long long K, size_t ws_bytes, int flags, int *tile_rows, int *splits, int *kb_per_split, int *ctas);
-int gemm3_dense_dispatch(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx,
-                         int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st);
-int gemm4_fused_dispatch(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
-                         long long ldx, int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes,
-                         int flags, const void *loraT, long long ldt, const void *loraU, cudaStream_t st);
-bool gemm4_supported(int type, const void *W, long long N, long long K);
-size_t gemm4_workspace(long long M, long long N, long long K, int flags);
-void gemm4_plan_info(long long M, long long N, long long K, size_t ws_bytes, int flags, int *tile_tokens, int *splits, int *spans_per_split, int *items);
-int gemv_max_m();
-bool gemv2_supported(int type, const void *W, long long N, long long K, long long M);
-int gemv2_dispatch(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype, const void *bias,
-                   int bias_dtype, void *Y, long long ldy, cudaStream_t st, bool w_stable = false);
-size_t repack_bytes(int type, long long N, long long K, int *pitch, long long *span_stride);
-int repack_dispatch(int type, const void *W, long long N, long long K, void *out, cudaStream_t st);
-}  // namespace ggufb200
+#include "internal.h"
 
 using namespace ggufb200;
 
 static bool type_geom(int t, int *bs, int *ts)
 {
-    int b = 0, s = 0;
-    switch (t) {
-    case T_Q4_0: b = 32; s = 18; break;
-    case T_Q4_1: b = 32; s = 20; break;
-    case T_Q5_0: b = 32; s = 22; break;
-    case T_Q5_1: b = 32; s = 24; break;
-    case T_Q8_0: b = 32; s = 34; break;
-    case T_Q2_K: b = 256; s = 84; break;
-    case T_Q3_K: b = 256; s = 110; break;
-    case T_Q4_K: b = 256; s = 144; break;
-    case T_Q5_K: b = 256; s = 176; break;
-    case T_Q6_K: b = 256; s = 210; break;
-    case T_IQ4_NL: b = 32; s = 18; break;
-    case T_IQ4_XS: b = 256; s = 136; break;
-    case T_BF16: b = 1; s = 2; break;
-    default: return false;
-    }
+    int b = 1, s = 2;       // BF16: one 2-byte element per "block"
+    const bool known = t == T_BF16 || with_block(t, false, [&](auto blk) {
+        b = decltype(blk)::BS;
+        s = decltype(blk)::TS;
+        return true;
+    });
+    if (!known) return false;
     if (bs) *bs = b;
     if (ts) *ts = s;
     return true;
@@ -96,29 +57,23 @@ struct Route {
     size_t ws;         // workspace bytes the route wants (0 = none)
 };
 
-// ABI flag bits -> gemm4's internal switches (1 = fast producers, 2 = 384-token items, 4 = no split-K)
-static int g4_flags(int flags)
+// GGUFB200_FLAG_* bits -> the options of the warpgroup-MMA routes (GENERIC wins over EXACT_W, TILE384 over TILE192)
+static LinearOptions linear_options(int flags)
 {
-    int f = (flags & GGUFB200_FLAG_GENERIC) ? 0 : 1;
-    if (flags & GGUFB200_FLAG_EXACT_W) f |= 16;       // hand-written producers that keep the reference's rounding sequence
-    if (flags & GGUFB200_FLAG_TILE384) f |= 2;
-    if (flags & GGUFB200_FLAG_TILE192) f |= 32;
-    if (flags & GGUFB200_FLAG_NOSPLIT) f |= 4;
-    return f;
-}
-
-static size_t fused_mma_ws(long long M, long long N, long long K, int flags)
-{
-    if (flags & GGUFB200_FLAG_NOSPLIT) return 0;
-    const int s = gemm2_fused_splits(M, N, K);
-    return s > 1 ? (size_t)s * (size_t)M * (size_t)N * 4 : 0;
+    LinearOptions o;
+    if (flags & GGUFB200_FLAG_GENERIC) o.producers = LinearOptions::GENERIC;
+    else if (flags & GGUFB200_FLAG_EXACT_W) o.producers = LinearOptions::EXACT;
+    if (flags & GGUFB200_FLAG_TILE384) o.tile = 384;
+    else if (flags & GGUFB200_FLAG_TILE192) o.tile = 192;
+    o.nosplit = (flags & GGUFB200_FLAG_NOSPLIT) != 0;
+    return o;
 }
 
 // `W` may be NULL (workspace query: assume a 16-byte aligned weight); ws_avail = workspace the caller supplied (SIZE_MAX in a query);
-// have_spans: the caller also holds the re-packed span-major copy of the weight (ggufb200_repack), which the TMEM-fed
-// kernel can stage for every block format and every K
-static Route pick_route(int type, const void *W, long long M, long long N, long long K, int act, int math, int algo_flags, size_t ws_avail,
-                        bool have_spans = false)
+// have_spans: the caller also holds the re-packed span-major copy of the weight (ggufb200_repack), which the FUSED_TMEM
+// kernel can read for every block format and every K
+static Route pick_route(int type, const void *W, long long M, long long N, long long K, int act, int math, int algo_flags,
+                        const LinearOptions &opt, size_t ws_avail, bool have_spans = false)
 {
     const int algo = algo_flags & GGUFB200_ALGO_MASK;
     const int flags = algo_flags & ~GGUFB200_ALGO_MASK;
@@ -135,7 +90,7 @@ static Route pick_route(int type, const void *W, long long M, long long N, long 
         //    fused reference-exact kernel's time at every M from 64 to 4608, so FUSED_MMA is only taken when the caller's
         //    workspace cannot hold the dequantised weight.
         // A math dtype other than fp16 means the reference's own sequence in that dtype: standalone dequant + dense GEMM (or the GEMV).
-        const bool tmem_ok = w_ok && fused_type(type) && math == kF16 && (N % 8) == 0 && (have_spans || gemm4_supported(type, W, N, K));
+        const bool tmem_ok = w_ok && fused_type(type) && math == kF16 && (N % 8) == 0 && (have_spans || fused_tmem_supported(type, W, N, K));
         const bool exact = (flags & GGUFB200_FLAG_EXACT_W) != 0 || math != kF16;
         if (!w_ok) r.algo = GGUFB200_ALGO_DEQUANT_MMA;
         else if (M <= gemv_max_m() && !exact && gemv2_supported(type, W ? W : (const void *)16, N, K, M)) r.algo = GGUFB200_ALGO_GEMV_FAST;
@@ -146,8 +101,8 @@ static Route pick_route(int type, const void *W, long long M, long long N, long 
     }
     switch (r.algo) {
     case GGUFB200_ALGO_DEQUANT_MMA: r.ws = dense; break;
-    case GGUFB200_ALGO_FUSED_MMA: r.ws = fusable ? fused_mma_ws(M, N, K, flags) : 0; break;
-    case GGUFB200_ALGO_FUSED_TMEM: r.ws = gemm4_workspace(M, N, K, g4_flags(flags)); break;
+    case GGUFB200_ALGO_FUSED_MMA: r.ws = fusable ? fused_mma_workspace(M, N, K, opt) : 0; break;
+    case GGUFB200_ALGO_FUSED_TMEM: r.ws = fused_tmem_workspace(M, N, K, opt); break;
     default: r.ws = 0;
     }
     (void)act;
@@ -252,7 +207,7 @@ int ggufb200_dequant_rows(int ggml_type, const void *packed, int64_t n_table_row
 size_t ggufb200_linear_workspace_ex(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int math_dtype, int algo)
 {
     if (!type_geom(ggml_type, nullptr, nullptr) || N <= 0 || K <= 0 || M <= 0) return 0;
-    return pick_route(ggml_type, nullptr, M, N, K, act_dtype, math_dtype, algo, (size_t)-1).ws;
+    return pick_route(ggml_type, nullptr, M, N, K, act_dtype, math_dtype, algo, linear_options(algo), (size_t)-1).ws;
 }
 
 size_t ggufb200_linear_workspace(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int algo)
@@ -278,6 +233,7 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
     if (M == 0) return GGUFB200_OK;
     if (!W_packed || !X || !Y) return GGUFB200_E_NULL;
     const int flags = algo & ~GGUFB200_ALGO_MASK;
+    const LinearOptions opt = linear_options(flags);
     const bool w_ok = aligned16(W_packed);
     const size_t dense = (size_t)N * (size_t)K * 2;
     const size_t ws_avail = (workspace && aligned16(workspace)) ? workspace_bytes : 0;
@@ -289,7 +245,7 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
         algo = GGUFB200_ALGO_DEQUANT_MMA | flags;
     }
     if (W_spans && !aligned16(W_spans)) return GGUFB200_E_ALIGN;
-    const Route r = pick_route(ggml_type, W_packed, M, N, K, act_dtype, math_dtype, algo, ws_avail, W_spans != nullptr);
+    const Route r = pick_route(ggml_type, W_packed, M, N, K, act_dtype, math_dtype, algo, opt, ws_avail, W_spans != nullptr);
     // the small-M kernel stores per element: it only needs 2-byte aligned Y rows; every other route moves 16-byte vectors
     const bool vec_y = r.algo != GGUFB200_ALGO_GEMV && r.algo != GGUFB200_ALGO_GEMV_FAST;
     if (!aligned16(X) || (ldx % 8) != 0) return GGUFB200_E_ALIGN;
@@ -309,25 +265,21 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
     case GGUFB200_ALGO_GEMV_FAST:
         if (math_dtype != kF16 || (flags & GGUFB200_FLAG_EXACT_W)) return GGUFB200_E_UNSUPPORTED;
         return gemv2_dispatch(ggml_type, W_packed, N, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st, (flags & GGUFB200_FLAG_W_STABLE) != 0);
-    case GGUFB200_ALGO_FUSED_MMA: {
-        if (!fused_type(ggml_type)) return GGUFB200_E_UNSUPPORTED;
-        int f = 0;
-        if (flags & GGUFB200_FLAG_NOSPLIT) f |= 1;
-        return gemm2_fused_dispatch(ggml_type, W_packed, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, workspace,
-                                    ws_avail, f, st);
-    }
+    case GGUFB200_ALGO_FUSED_MMA:
+        if (!fused_type(ggml_type) || math_dtype != kF16) return GGUFB200_E_UNSUPPORTED;
+        return fused_mma_linear(ggml_type, W_packed, N, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, workspace, ws_avail, opt, st);
     case GGUFB200_ALGO_FUSED_TMEM: {
         if (!fused_type(ggml_type) || math_dtype != kF16) return GGUFB200_E_UNSUPPORTED;
         long long span_stride = 0;
         if (W_spans) repack_bytes(ggml_type, N, K, nullptr, &span_stride);
-        return gemm4_fused_dispatch(ggml_type, W_packed, W_spans, span_stride, N, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, workspace,
-                                    ws_avail, g4_flags(flags), lora ? lora->T : nullptr, lora ? lora->ldt : 0, lora ? lora->U : nullptr, st);
+        return fused_tmem_linear(ggml_type, W_packed, W_spans, span_stride, N, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, workspace,
+                                 ws_avail, opt, lora ? lora->T : nullptr, lora ? lora->ldt : 0, lora ? lora->U : nullptr, st);
     }
     case GGUFB200_ALGO_DEQUANT_MMA: {
         if (ws_avail < dense) return GGUFB200_E_WORKSPACE;
         int rc = dequant_dispatch(ggml_type, W_packed, N * (K / bs), workspace, act_dtype, math_dtype, st, (flags & GGUFB200_FLAG_W_STABLE) != 0);
         if (rc != GGUFB200_OK) return rc;
-        return gemm3_dense_dispatch(workspace, N, K, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st);
+        return dense_gemm(workspace, N, K, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st);
     }
     }
     return GGUFB200_E_UNSUPPORTED;
@@ -383,15 +335,15 @@ int ggufb200_linear_plan(int ggml_type, int64_t M, int64_t N, int64_t K, size_t 
     if (!tile_rows || !k_ranges || !kblocks_per_range || !ctas) return GGUFB200_E_NULL;
     if (M <= 0 || N <= 0 || K <= 0 || K % 64 != 0 || N % 8 != 0) return GGUFB200_E_SHAPE;
     if (!fused_type(ggml_type)) return GGUFB200_E_UNSUPPORTED;
-    const int flags = algo & ~GGUFB200_ALGO_MASK;
+    const LinearOptions opt = linear_options(algo);
     if ((algo & GGUFB200_ALGO_MASK) == GGUFB200_ALGO_FUSED_TMEM) {
         int spans = 1;
-        gemm4_plan_info(M, N, K, workspace_bytes, g4_flags(flags), tile_rows, k_ranges, &spans, ctas);
+        fused_tmem_plan(M, N, K, workspace_bytes, opt, tile_rows, k_ranges, &spans, ctas);
         *kblocks_per_range = 4 * spans;
         return GGUFB200_OK;
     }
     if ((algo & GGUFB200_ALGO_MASK) != GGUFB200_ALGO_FUSED_MMA) return GGUFB200_E_UNSUPPORTED;
-    gemm2_fused_plan_info(M, N, K, workspace_bytes, (flags & GGUFB200_FLAG_NOSPLIT) ? 1 : 0, tile_rows, k_ranges, kblocks_per_range, ctas);
+    fused_mma_plan(M, N, K, workspace_bytes, opt, tile_rows, k_ranges, kblocks_per_range, ctas);
     return GGUFB200_OK;
 }
 
@@ -405,7 +357,7 @@ int ggufb200_gemm(const void *W, int64_t N, int64_t K, int64_t ldw, const void *
     if (!W || !X || !Y) return GGUFB200_E_NULL;
     if (!aligned16(W) || !aligned16(X) || !aligned16(Y) || (ldw % 8) || (ldx % 8) || (ldy % 8)) return GGUFB200_E_ALIGN;
     if (int rc = device_check()) return rc;
-    return gemm3_dense_dispatch(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, (cudaStream_t)stream);
+    return dense_gemm(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -26,6 +26,10 @@ enum : int {
     T_Q5_K = 13, T_Q6_K = 14, T_IQ4_NL = 20, T_IQ4_XS = 23, T_BF16 = 30
 };
 
+// The 12 block formats (every type above but BF16), X(T) once each.  Dispatch sites go through with_block() below.
+#define GGUFB200_BLOCK_TYPES(X) \
+    X(T_Q4_0) X(T_Q4_1) X(T_Q5_0) X(T_Q5_1) X(T_Q8_0) X(T_Q2_K) X(T_Q3_K) X(T_Q4_K) X(T_Q5_K) X(T_Q6_K) X(T_IQ4_NL) X(T_IQ4_XS)
+
 // spread the low four bits of t over the low bit of four bytes (bit i -> byte i)
 GG_HD uint32_t spread4(uint32_t t) { return ((t & 0xFu) * 0x00204081u) & 0x01010101u; }
 
@@ -368,6 +372,18 @@ GG_HD void dequant_run(const uint8_t *blk, int e0, typename Math<MATH>::T2 (&out
 {
     const GroupScale<MATH> g = group_scale<Q, MATH>(blk, e0);
     dequant_elems<Q, MATH, N>(blk, e0, g, out);
+}
+
+// Host-side dispatch on a ggml type code: f(Block<T>{}) for a block format, `other` for BF16 and unknown codes.
+template <class R, class F> R with_block(int type, R other, F &&f)
+{
+    switch (type) {
+#define GGUFB200_BLOCK_CASE(T) \
+    case T: return f(Block<T>{});
+        GGUFB200_BLOCK_TYPES(GGUFB200_BLOCK_CASE)
+#undef GGUFB200_BLOCK_CASE
+    }
+    return other;
 }
 
 }  // namespace ggufb200

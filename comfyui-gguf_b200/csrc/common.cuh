@@ -165,7 +165,6 @@ template <int A> GG_HD uint32_t ld16(const uint8_t *p)
         return (uint32_t)p[0] | ((uint32_t)p[1] << 8);
     }
 }
-constexpr __host__ __device__ int gcd_int(int a, int b) { return b == 0 ? a : gcd_int(b, a % b); }
 
 // ------------------------------------------------------------------ math policies
 // T  : one value in the math dtype;  T2 : two values.

@@ -16,6 +16,7 @@
 //     tile in shared memory, which leaves through ONE swizzled tensor-map store (cp.async.bulk.tensor.2d, SASS UTMASTG): no
 //     thread computes a global address, every HBM write is a full line, and the unpack runs with immediate offsets
 #include "blocks.cuh"
+#include "internal.h"
 #include "wgmma.cuh"
 
 namespace ggufb200 {
@@ -209,7 +210,7 @@ template <class Q, int MATH, int OUT> static int launch_dequant(const void *pack
     CUtensorMap tmOut{};
     {
         // the output as [runs of 32 elements][64 | 128 bytes]: one row per thread, one box of THREADS rows per tile
-        G2EncodeFn fn = g2_encode_fn();
+        TensorMapEncodeFn fn = tensor_map_encode_fn();
         const long long n_rows = n_blocks * (long long)Q::BS / 32;
         if (!fn || n_rows > 0x7fffffffll) return GGUFB200_E_CUDA;
         cuuint64_t dims[2] = {(cuuint64_t)(32 * OB), (cuuint64_t)n_rows};
@@ -260,20 +261,7 @@ template <class Q> static int dispatch_math(const void *packed, long long n_bloc
 int dequant_dispatch(int type, const void *packed, long long n_blocks, void *out, int out_dtype, int math_dtype, cudaStream_t st, bool stable)
 {
     if (n_blocks == 0) return GGUFB200_OK;
-    switch (type) {
-    case T_Q4_0: return dispatch_math<Block<T_Q4_0>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q4_1: return dispatch_math<Block<T_Q4_1>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q5_0: return dispatch_math<Block<T_Q5_0>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q5_1: return dispatch_math<Block<T_Q5_1>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q8_0: return dispatch_math<Block<T_Q8_0>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q2_K: return dispatch_math<Block<T_Q2_K>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q3_K: return dispatch_math<Block<T_Q3_K>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q4_K: return dispatch_math<Block<T_Q4_K>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q5_K: return dispatch_math<Block<T_Q5_K>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_Q6_K: return dispatch_math<Block<T_Q6_K>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_IQ4_NL: return dispatch_math<Block<T_IQ4_NL>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_IQ4_XS: return dispatch_math<Block<T_IQ4_XS>>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
-    case T_BF16: {
+    if (type == T_BF16) {
         // one 8-element vector per thread, CTAs in address order (the grid-stride loop of the kernel only runs past the first
         // iteration for tensors beyond 2^31 CTAs): same reasoning as for the block formats above
         long long blocks = (n_blocks + (long long)kThreads * 8 - 1) / ((long long)kThreads * 8);
@@ -286,8 +274,9 @@ int dequant_dispatch(int type, const void *packed, long long n_blocks, void *out
         else return GGUFB200_E_DTYPE;
         return cudaGetLastError() == cudaSuccess ? GGUFB200_OK : GGUFB200_E_CUDA;
     }
-    }
-    return GGUFB200_E_TYPE;
+    return with_block(type, GGUFB200_E_TYPE, [&](auto blk) {
+        return dispatch_math<decltype(blk)>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
+    });
 }
 
 template <class Q> static int launch_unpack(const void *packed, long long n_blocks, int16_t *q, int16_t *sc, int16_t *mn, cudaStream_t st)
@@ -302,21 +291,7 @@ template <class Q> static int launch_unpack(const void *packed, long long n_bloc
 int unpack_dispatch(int type, const void *packed, long long n_blocks, int16_t *q, int16_t *sc, int16_t *mn, cudaStream_t st)
 {
     if (n_blocks == 0) return GGUFB200_OK;
-    switch (type) {
-    case T_Q4_0: return launch_unpack<Block<T_Q4_0>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q4_1: return launch_unpack<Block<T_Q4_1>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q5_0: return launch_unpack<Block<T_Q5_0>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q5_1: return launch_unpack<Block<T_Q5_1>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q8_0: return launch_unpack<Block<T_Q8_0>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q2_K: return launch_unpack<Block<T_Q2_K>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q3_K: return launch_unpack<Block<T_Q3_K>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q4_K: return launch_unpack<Block<T_Q4_K>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q5_K: return launch_unpack<Block<T_Q5_K>>(packed, n_blocks, q, sc, mn, st);
-    case T_Q6_K: return launch_unpack<Block<T_Q6_K>>(packed, n_blocks, q, sc, mn, st);
-    case T_IQ4_NL: return launch_unpack<Block<T_IQ4_NL>>(packed, n_blocks, q, sc, mn, st);
-    case T_IQ4_XS: return launch_unpack<Block<T_IQ4_XS>>(packed, n_blocks, q, sc, mn, st);
-    }
-    return GGUFB200_E_TYPE;
+    return with_block(type, GGUFB200_E_TYPE, [&](auto blk) { return launch_unpack<decltype(blk)>(packed, n_blocks, q, sc, mn, st); });
 }
 
 }  // namespace ggufb200

@@ -7,6 +7,7 @@
 // W is rounded to the activation dtype exactly as the reference does before F.linear
 // (dequant.py:23, ops.py:210) and accumulated in fp32; warp-shuffle reduction at the end.
 #include "blocks.cuh"
+#include "internal.h"
 
 namespace ggufb200 {
 
@@ -253,20 +254,7 @@ int gemv_dispatch(int type, const void *W, long long N, long long K, const void 
                   const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st)
 {
     if (M > kGemvMaxM) return GGUFB200_E_SHAPE;
-    switch (type) {
-    case T_Q4_0: return gemv_math<Block<T_Q4_0>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q4_1: return gemv_math<Block<T_Q4_1>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q5_0: return gemv_math<Block<T_Q5_0>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q5_1: return gemv_math<Block<T_Q5_1>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q8_0: return gemv_math<Block<T_Q8_0>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q2_K: return gemv_math<Block<T_Q2_K>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q3_K: return gemv_math<Block<T_Q3_K>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q4_K: return gemv_math<Block<T_Q4_K>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q5_K: return gemv_math<Block<T_Q5_K>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_Q6_K: return gemv_math<Block<T_Q6_K>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_IQ4_NL: return gemv_math<Block<T_IQ4_NL>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_IQ4_XS: return gemv_math<Block<T_IQ4_XS>>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
-    case T_BF16: {
+    if (type == T_BF16) {
         const uint16_t *w = reinterpret_cast<const uint16_t *>(W);
         const uint8_t *x = reinterpret_cast<const uint8_t *>(X);
         uint8_t *y = reinterpret_cast<uint8_t *>(Y);
@@ -275,8 +263,9 @@ int gemv_dispatch(int type, const void *W, long long N, long long K, const void 
         else gemv_bf16w_kernel<kF16, 8><<<grid, kGemvThreads, 0, st>>>(w, N, K, x, ldx, (int)M, bias, bias_dtype, y, ldy);
         return cudaGetLastError() == cudaSuccess ? GGUFB200_OK : GGUFB200_E_CUDA;
     }
-    }
-    return GGUFB200_E_TYPE;
+    return with_block(type, GGUFB200_E_TYPE, [&](auto blk) {
+        return gemv_math<decltype(blk)>(W, N, K, X, M, ldx, act_dtype, math_dtype, bias, bias_dtype, Y, ldy, st);
+    });
 }
 
 }  // namespace ggufb200

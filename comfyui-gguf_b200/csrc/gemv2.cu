@@ -24,6 +24,7 @@
 // tiles are reduced through a double-buffered shared-memory tile at the end of a row tile (one named barrier per tile).  The
 // activations (<= 8 rows) are staged once per CTA by bulk copies, their sub-block sums computed once per CTA from that copy.
 #include "blocks.cuh"
+#include "internal.h"
 #include "wgmma.cuh"
 
 namespace ggufb200 {
@@ -359,7 +360,7 @@ __global__ void __launch_bounds__(kV2Threads) gemv2_kernel(const __grid_constant
 // [N][K / 256][TS] bytes as a 3-D tensor: one box = 16 rows x 6 super-blocks, dense in shared memory
 template <int TS> static bool v2_make_map(CUtensorMap *tm, const void *W, long long N, long long K)
 {
-    G2EncodeFn fn = g2_encode_fn();
+    TensorMapEncodeFn fn = tensor_map_encode_fn();
     if (!fn) return false;
     cuuint64_t dims[3] = {(cuuint64_t)TS, (cuuint64_t)(K / 256), (cuuint64_t)N};
     cuuint64_t strides[2] = {(cuuint64_t)TS, (cuuint64_t)(K / 256 * TS)};

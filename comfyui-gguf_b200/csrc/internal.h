@@ -1,0 +1,63 @@
+// internal.h -- every function api.cu calls in another translation unit, and the two tuning globals.  api.cu and each file
+// that defines one of these include this header, so a changed signature fails to compile instead of to link, and default
+// arguments are written here only.
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+
+namespace ggufb200 {
+
+// ------------------------------------------------------------------ tuning switches (ggufb200_set_tuning)
+extern int g_dequant_pdl;      // dequant.cu: programmatic dependent launch of the dequant kernel (key 1)
+extern int g_gemv2_ctas;       // gemv2.cu: CTAs per SM of the integer-pattern GEMV, 0 = pick (key 2)
+
+// ------------------------------------------------------------------ dequant.cu, rows.cu
+int dequant_dispatch(int type, const void *packed, long long n_blocks, void *out, int out_dtype, int math_dtype, cudaStream_t st, bool stable = false);
+int unpack_dispatch(int type, const void *packed, long long n_blocks, int16_t *q, int16_t *sc, int16_t *mn, cudaStream_t st);
+int rows_dispatch(int type, const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows, void *out,
+                  int out_dtype, int math_dtype, cudaStream_t st);
+
+// ------------------------------------------------------------------ small-M Linear: gemv.cu (GGUFB200_ALGO_GEMV), gemv2.cu (GEMV_FAST)
+int gemv_max_m();
+int gemv_dispatch(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype, int math_dtype,
+                  const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st);
+bool gemv2_supported(int type, const void *W, long long N, long long K, long long M);
+int gemv2_dispatch(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype, const void *bias,
+                   int bias_dtype, void *Y, long long ldy, cudaStream_t st, bool w_stable = false);
+
+// ------------------------------------------------------------------ repack.cu: the span-major copy of a packed weight
+size_t repack_bytes(int type, long long N, long long K, int *pitch, long long *span_stride);
+int repack_dispatch(int type, const void *W, long long N, long long K, void *out, cudaStream_t st);
+
+// ------------------------------------------------------------------ linear_sm90.cu: the warpgroup-MMA Linear
+// Per-call options of the fused routes, decoded once from the GGUFB200_FLAG_* bits (api.cu).
+struct LinearOptions {
+    enum Producers { FAST, EXACT, GENERIC };
+    Producers producers = FAST;    // FUSED_TMEM weight producers: hand-written with one fused multiply-add per element (FAST),
+                                   // hand-written with the reference's rounding sequence (EXACT), functor producers (GENERIC)
+    int tile = 0;                  // FUSED_TMEM token items: 0 = the cost model picks, 192 or 384 = forced
+    bool nosplit = false;          // never cut K into ranges
+};
+
+// `ws_bytes` is the usable workspace at `ws`: 0 when the caller passed none or a misaligned one.
+// Dense GEMM: ggufb200_gemm and the GEMM half of GGUFB200_ALGO_DEQUANT_MMA.
+int dense_gemm(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx, int act_dtype,
+               const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st);
+// GGUFB200_ALGO_FUSED_MMA: reference-exact producers, the weight as the wide operand.
+size_t fused_mma_workspace(long long M, long long N, long long K, const LinearOptions &opt);
+void fused_mma_plan(long long M, long long N, long long K, size_t ws_bytes, const LinearOptions &opt, int *tile_rows, int *splits,
+                    int *kb_per_split, int *ctas);
+int fused_mma_linear(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype,
+                     const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes, const LinearOptions &opt,
+                     cudaStream_t st);
+// GGUFB200_ALGO_FUSED_TMEM: the transposed product, token tiles sized to the activation, optional LoRA k-block.
+bool fused_tmem_supported(int type, const void *W, long long N, long long K);
+size_t fused_tmem_workspace(long long M, long long N, long long K, const LinearOptions &opt);
+void fused_tmem_plan(long long M, long long N, long long K, size_t ws_bytes, const LinearOptions &opt, int *tile_tokens, int *splits,
+                     int *spans_per_split, int *items);
+int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
+                      long long ldx, int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes,
+                      const LinearOptions &opt, const void *loraT, long long ldt, const void *loraU, cudaStream_t st);
+
+}  // namespace ggufb200

@@ -1,5 +1,5 @@
-// linear_sm90.cuh -- the warpgroup-MMA Linear kernel shared by the dense GEMM (gemm3.cu), the smem-fed fused kernel
-// (gemm2.cu) and the span-fed fused kernel (gemm4.cu).
+// linear_sm90.cuh -- the warpgroup-MMA Linear kernel behind the dense GEMM, GGUFB200_ALGO_FUSED_MMA and
+// GGUFB200_ALGO_FUSED_TMEM; their launchers are in linear_sm90.cu.
 //
 //   Y[M,N] = X[M,K] * W[N,K]^T (+ bias)      X fp16 / bf16, W dense (TMA) or packed GGUF rows dequantised on chip, fp32 accumulation
 //
@@ -114,8 +114,8 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
             const bool lora_kb = i == nkb_main;                // the extra k-block: X -> T = x * down^T, W -> U = scale * up
             if (t == 0) {
                 mbar_arrive_expect_tx(&full[s], TOK * 128 + (DENSE ? WROWS * 128 : 0));
-                tma_load_2d(x_tile, lora_kb ? &tmT : &tmX, &full[s], lora_kb ? 0 : kb * kG2BK, (int)tok0);
-                if constexpr (DENSE) tma_load_2d(w_tile, &tmW, &full[s], kb * kG2BK, (int)feat0);
+                tma_load_2d(x_tile, lora_kb ? &tmT : &tmX, &full[s], lora_kb ? 0 : kb * kBlockK, (int)tok0);
+                if constexpr (DENSE) tma_load_2d(w_tile, &tmW, &full[s], kb * kBlockK, (int)feat0);
             }
             if constexpr (!DENSE) {
 #pragma unroll 1
@@ -130,7 +130,7 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                                          wg_h2_to_act<ACT>(o[4 * c + 2]), wg_h2_to_act<ACT>(o[4 * c + 3]));
                         }
                     };
-                    if (n >= p.N || (!lora_kb && (long long)kb * kG2BK >= p.K)) {
+                    if (n >= p.N || (!lora_kb && (long long)kb * kBlockK >= p.K)) {
 #pragma unroll
                         for (int c = 0; c < 8; ++c) st_shared_v4(dst + (uint32_t)(c << 4), 0, 0, 0, 0);
                     } else if (lora_kb) {
@@ -175,7 +175,7 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         const uint64_t da = wg_desc_sw128(a_addr), db = wg_desc_sw128(b_addr);
         wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < kG2BK / 16; ++j) Wgmma<ACT, TN>::mma(acc, da + (uint64_t)(2 * j), db + (uint64_t)(2 * j));
+        for (int j = 0; j < kBlockK / 16; ++j) Wgmma<ACT, TN>::mma(acc, da + (uint64_t)(2 * j), db + (uint64_t)(2 * j));
         wgmma_commit();
         if (i > 0) {
             wgmma_wait<1>();                                   // k-block i-1 has been read: hand its stage back
@@ -213,7 +213,7 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                 const int ar = arow0 + 8 * h, bc = 8 * j + bcol0 + e;
                 const int tk = TRANS ? bc : ar, f = TRANS ? ar : bc;
                 float v = acc[4 * j + 2 * h + e];
-                if (p.bias && feat0 + f < p.N) v += g2_bias<ACT>(p.bias, p.bias_dtype, feat0 + f);
+                if (p.bias && feat0 + f < p.N) v += wg_bias<ACT>(p.bias, p.bias_dtype, feat0 + f);
                 uint16_t hb;
                 if constexpr (ACT == kBF16) hb = __bfloat16_as_ushort(__float2bfloat16_rn(v));
                 else hb = __half_as_ushort(__float2half_rn(v));
@@ -263,9 +263,9 @@ __global__ void __launch_bounds__(256) wg_finalize_kernel(const float *__restric
         }
         if (bias) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) v[j] += g2_bias<ACT>(bias, bias_dtype, n + j);
+            for (int j = 0; j < 8; ++j) v[j] += wg_bias<ACT>(bias, bias_dtype, n + j);
         }
-        st_global_v4(Y + (m * ldy + n) * 2, g2_pack<ACT>(v[0], v[1]), g2_pack<ACT>(v[2], v[3]), g2_pack<ACT>(v[4], v[5]), g2_pack<ACT>(v[6], v[7]));
+        st_global_v4(Y + (m * ldy + n) * 2, wg_pack<ACT>(v[0], v[1]), wg_pack<ACT>(v[2], v[3]), wg_pack<ACT>(v[4], v[5]), wg_pack<ACT>(v[6], v[7]));
     }
 }
 

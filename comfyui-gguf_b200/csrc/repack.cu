@@ -1,10 +1,10 @@
-// repack.cu -- one-time re-layout of a packed GGUF weight into the SPAN-MAJOR shadow layout the TMEM-fed fused kernel
-// (gemm4.cu) can stage with ONE bulk async copy per tile, whatever the block size is (SURVEY 8f rank 3).
+// repack.cu -- one-time re-layout of a packed GGUF weight into the SPAN-MAJOR shadow layout whose rows the producers of
+// GGUFB200_ALGO_FUSED_TMEM (linear_sm90.cu) read with 16-byte loads, whatever the block size is (SURVEY 8f rank 3).
 //
 // Canonical layout (loader.py:96-120, gguf-py): N rows of K/bs blocks, row stride = K/bs*ts bytes.  Block sizes of
 // 84 / 110 / 136 / 210 bytes (Q2_K / Q3_K / IQ4_XS / Q6_K) and row strides that are not multiples of 16 bytes (Q8_0 at
-// K = 2432: 2584 B) make 2-D tensor maps over the raw bytes illegal, so those weights could only use the direct-load
-// producers.  Shadow layout:
+// K = 2432: 2584 B) leave a row's span without 16-byte alignment, so the FUSED_TMEM producers cannot read those weights
+// from the canonical rows.  Shadow layout:
 //
 //     out[s][n][PITCH]      s = 256-wide K-span index (ceil(K/256)), n = row index padded to a multiple of 256,
 //                           PITCH = SpanOf<Q>::PITCH >= the span's packed bytes, a multiple of 16 (odd multiple of 16
@@ -13,6 +13,7 @@
 // The 128 rows of one CTA for one span are then 128*PITCH contiguous, 16-byte aligned bytes.  Pad bytes, rows >= N and the
 // tail of a ragged last span are zero (a zero block dequantises to 0 in every format).  The canonical bytes stay where
 // they are: GGMLTensor / state_dict semantics are untouched, the shadow is a cache the host layer may drop at any time.
+#include "internal.h"
 #include "produce.cuh"
 
 namespace ggufb200 {
@@ -50,19 +51,11 @@ template <class Q> static int repack_run(const void *W, long long N, long long K
     return cudaGetLastError() == cudaSuccess ? GGUFB200_OK : GGUFB200_E_CUDA;
 }
 
-#define GGUFB200_REPACK_TYPES(X) \
-    X(T_Q4_0) X(T_Q4_1) X(T_Q5_0) X(T_Q5_1) X(T_Q8_0) X(T_Q2_K) X(T_Q3_K) X(T_Q4_K) X(T_Q5_K) X(T_Q6_K) X(T_IQ4_NL) X(T_IQ4_XS)
-
 // bytes of the shadow buffer and its geometry; 0 for types without a block layout
 size_t repack_bytes(int type, long long N, long long K, int *pitch, long long *span_stride)
 {
-    int pt = 0;
-    switch (type) {
-#define X(T) case T: pt = SpanOf<Block<T>>::PITCH; break;
-        GGUFB200_REPACK_TYPES(X)
-#undef X
-    default: return 0;
-    }
+    const int pt = with_block(type, 0, [](auto blk) { return SpanOf<decltype(blk)>::PITCH; });
+    if (pt == 0) return 0;
     const long long n_pad = (N + 255) / 256 * 256;
     if (pitch) *pitch = pt;
     if (span_stride) *span_stride = n_pad * pt;
@@ -71,12 +64,7 @@ size_t repack_bytes(int type, long long N, long long K, int *pitch, long long *s
 
 int repack_dispatch(int type, const void *W, long long N, long long K, void *out, cudaStream_t st)
 {
-    switch (type) {
-#define X(T) case T: return repack_run<Block<T>>(W, N, K, out, st);
-        GGUFB200_REPACK_TYPES(X)
-#undef X
-    }
-    return GGUFB200_E_TYPE;
+    return with_block(type, GGUFB200_E_TYPE, [&](auto blk) { return repack_run<decltype(blk)>(W, N, K, out, st); });
 }
 
 }  // namespace ggufb200

@@ -4,6 +4,7 @@
 // table on every call and then runs F.embedding: here only the requested rows are read
 // (K/BS*TS bytes each) and written (K elements each).  One CTA per (row, 2048-element chunk).
 #include "blocks.cuh"
+#include "internal.h"
 
 namespace ggufb200 {
 
@@ -114,20 +115,7 @@ static int rows_math(const void *p, long long nt, long long K, const long long *
 int rows_dispatch(int type, const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows, void *out,
                   int out_dtype, int math_dtype, cudaStream_t st)
 {
-    switch (type) {
-    case T_Q4_0: return rows_math<Block<T_Q4_0>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q4_1: return rows_math<Block<T_Q4_1>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q5_0: return rows_math<Block<T_Q5_0>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q5_1: return rows_math<Block<T_Q5_1>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q8_0: return rows_math<Block<T_Q8_0>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q2_K: return rows_math<Block<T_Q2_K>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q3_K: return rows_math<Block<T_Q3_K>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q4_K: return rows_math<Block<T_Q4_K>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q5_K: return rows_math<Block<T_Q5_K>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_Q6_K: return rows_math<Block<T_Q6_K>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_IQ4_NL: return rows_math<Block<T_IQ4_NL>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_IQ4_XS: return rows_math<Block<T_IQ4_XS>>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
-    case T_BF16: {
+    if (type == T_BF16) {
         for (long long y0 = 0; y0 < n_rows; y0 += 65535) {
             long long ny = n_rows - y0 < 65535 ? n_rows - y0 : 65535;
             dim3 grid((unsigned)((K + kRowThreads * 4 - 1) / (kRowThreads * 4)), (unsigned)ny);
@@ -138,8 +126,9 @@ int rows_dispatch(int type, const void *packed, long long n_table_rows, long lon
         }
         return cudaGetLastError() == cudaSuccess ? GGUFB200_OK : GGUFB200_E_CUDA;
     }
-    }
-    return GGUFB200_E_TYPE;
+    return with_block(type, GGUFB200_E_TYPE, [&](auto blk) {
+        return rows_math<decltype(blk)>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
+    });
 }
 
 }  // namespace ggufb200

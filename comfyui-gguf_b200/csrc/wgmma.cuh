@@ -8,7 +8,7 @@
 
 namespace ggufb200 {
 
-constexpr int kG2BK = 64;           // k-block: one 128-byte swizzle atom row of 16-bit elements
+constexpr int kBlockK = 64;           // k-block: one 128-byte swizzle atom row of 16-bit elements
 
 // 2-D TMA tile load global -> shared, completion bytes credited to an mbarrier of this CTA
 __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *tm, uint64_t *bar, int c0, int c1)
@@ -103,7 +103,7 @@ template <> struct Wgmma<kBF16, 256> {
     }
 };
 
-template <int ACT> __device__ __forceinline__ float g2_bias(const void *bias, int bias_dtype, long long n)
+template <int ACT> __device__ __forceinline__ float wg_bias(const void *bias, int bias_dtype, long long n)
 {
     float b;
     if (bias_dtype == kF32) b = reinterpret_cast<const float *>(bias)[n];
@@ -112,7 +112,7 @@ template <int ACT> __device__ __forceinline__ float g2_bias(const void *bias, in
     if constexpr (ACT == kBF16) return __bfloat162float(__float2bfloat16_rn(b));   // ops.py: bias is cast to x.dtype first
     else return __half2float(__float2half_rn(b));
 }
-template <int ACT> __device__ __forceinline__ uint32_t g2_pack(float a, float b)
+template <int ACT> __device__ __forceinline__ uint32_t wg_pack(float a, float b)
 {
     if constexpr (ACT == kBF16) {
         __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
@@ -124,31 +124,31 @@ template <int ACT> __device__ __forceinline__ uint32_t g2_pack(float a, float b)
 }
 
 // ------------------------------------------------------------------ host side
-typedef CUresult (*G2EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
+typedef CUresult (*TensorMapEncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
                                CUtensorMapFloatOOBfill);
 
-static inline G2EncodeFn g2_encode_fn()
+static inline TensorMapEncodeFn tensor_map_encode_fn()
 {
-    static G2EncodeFn fn = nullptr;
+    static TensorMapEncodeFn fn = nullptr;
     if (!fn) {
         void *ptr = nullptr;
         cudaDriverEntryPointQueryResult q;
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<G2EncodeFn>(ptr);
+            fn = reinterpret_cast<TensorMapEncodeFn>(ptr);
     }
     return fn;
 }
 
 // [rows, K] 16-bit matrix with row stride ld (elements), boxes of box_rows x 64, 128-byte swizzle; out-of-range rows and
 // columns of a box are zero-filled
-static inline bool g2_make_map(CUtensorMap *tm, const void *base, long long rows, long long K, long long ld, int act, int box_rows = 128)
+static inline bool make_kblock_map(CUtensorMap *tm, const void *base, long long rows, long long K, long long ld, int act, int box_rows = 128)
 {
-    G2EncodeFn fn = g2_encode_fn();
+    TensorMapEncodeFn fn = tensor_map_encode_fn();
     if (!fn) return false;
     cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-    cuuint32_t box[2] = {(cuuint32_t)kG2BK, (cuuint32_t)box_rows};
+    cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUtensorMapDataType dt = act == kBF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
     return fn(tm, dt, 2, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,

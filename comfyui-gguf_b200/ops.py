@@ -434,8 +434,8 @@ class GGMLOps(comfy_ops.manual_cast):
                 return None
             return terms
 
-        # LoRA inside the fused kernel (csrc/gemm4.cu: one extra k-block, SURVEY 8f rank 1): U = scale * up (fp16 [N, 64]) and
-        # down (act dtype [64, K]), zero padded to rank 64 and cached per patch set; per forward only T = x * down^T
+        # LoRA inside the fused kernel (GGUFB200_ALGO_FUSED_TMEM, csrc/linear_sm90.cu: one extra k-block, SURVEY 8f rank 1):
+        # U = scale * up (fp16 [N, 64]) and down (act dtype [64, K]), zero padded to rank 64 and cached per patch set; per forward only T = x * down^T
         # ([M, 64], this package's dense tensor-core GEMM) is computed before the fused call.
         # False -> the unpatched fused kernel plus two library GEMMs of rank sum(r) (`_add_lora`).
         lora_in_kernel = True

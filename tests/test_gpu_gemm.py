@@ -1,5 +1,5 @@
-"""GPU parity tests of the tensor-core Linear kernels: dense TMA-fed GEMM (csrc/gemm3.cu), the shared-memory-fed fused
-kernel (csrc/gemm2.cu, reference-exact W) and the FUSED_TMEM kernel (csrc/gemm4.cu, the AUTO default).
+"""GPU parity tests of the warpgroup-MMA Linear (csrc/linear_sm90.cu): the dense TMA-fed GEMM, GGUFB200_ALGO_FUSED_MMA
+(reference-exact W) and GGUFB200_ALGO_FUSED_TMEM (the AUTO default).
 
 Reference: fp32-accumulated x @ W^T (+bias) rounded to the activation dtype, where W is the bit-exact dequantised weight
 (validated separately against the reference's golden outputs).
@@ -87,7 +87,7 @@ def test_fused_gemm_all_types(pkg, qt, dt, staged):
 @pytest.mark.parametrize("qt", [Q.Q4_K, Q.Q8_0, Q.Q6_K, Q.Q5_0], ids=lambda q: q.name)
 @pytest.mark.parametrize("M,N,K", [(64, 512, 4096), (300, 264, 2048), (513, 520, 1280), (1000, 256, 5120), (24, 1032, 768)])
 def test_fused_gemm_split_k(pkg, qt, M, N, K):
-    """Short activations: the fused kernel cuts K into ranges of whole 256-wide spans, one SM pair per (tile, range), keeps
+    """Short activations: the fused kernel cuts K into ranges of whole 256-wide spans, one CTA per (tile, range), keeps
     fp32 partial tiles in the workspace and sums them in a fixed order (bit-reproducible).  Checked against the reference
     arithmetic and against the unsplit kernel (same tiles, no workspace): the two may differ only by fp32 summation order."""
     L = pkg.lib.lib()
@@ -96,7 +96,7 @@ def test_fused_gemm_split_k(pkg, qt, M, N, K):
     x = torch.randn(M, K, device=DEV, dtype=torch.bfloat16)
     b = torch.randn(N, device=DEV) * 0.1
     need = L.ggufb200_linear_workspace(int(qt), M, N, K, 1, pkg.lib.ALGO_FUSED_MMA)
-    assert need % (M * N * 4) == 0 and need >= 2 * M * N * 4, "these shapes leave SM pairs idle without split-K"
+    assert need % (M * N * 4) == 0 and need >= 2 * M * N * 4, "these shapes leave SMs idle without split-K"
     y = pkg.ops.linear_packed(x, w, b, None, pkg.lib.ALGO_FUSED_MMA)
     assert torch.equal(y, pkg.ops.linear_packed(x, w, b, None, pkg.lib.ALGO_FUSED_MMA)), "split-K must be reproducible"
     nosplit = pkg.lib.ALGO_FUSED_MMA | pkg.lib.FLAG_NOSPLIT
@@ -167,7 +167,7 @@ def test_fused_gemm_flux_shapes_q4k(pkg, M, N, K):
         assert err_ours <= 1.05 * err_ref, (algo, err_ours, err_ref)
 
 
-# ---------------------------------------------------------------- FUSED_TMEM kernel (csrc/gemm4.cu)
+# ---------------------------------------------------------------- FUSED_TMEM kernel (csrc/linear_sm90.cu)
 PRODUCERS = {"fast": 0, "generic": 0x200, "exact": 0x100}      # default / GGUFB200_FLAG_GENERIC / GGUFB200_FLAG_EXACT_W
 
 

@@ -1,4 +1,4 @@
-"""GPU parity tests of the Linear path (csrc/gemv.cu, gemm2.cu, gemm3.cu, gemm4.cu) through the plugin surface.
+"""GPU parity tests of the Linear path (csrc/gemv.cu, gemv2.cu, linear_sm90.cu) through the plugin surface.
 
 Tolerance (written here, from BASELINE.json north_star): ||y - y_ref||_F / ||y_ref||_F <= 1e-3 for fp16/bf16 Linear
 outputs; y_ref is the unmodified reference's GGMLOps.Linear output (golden files) or the CPU oracle.

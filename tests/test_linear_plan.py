@@ -1,4 +1,5 @@
-"""Host arithmetic of the fused Linear's tiling (csrc/gemm2.cu::g2_fused_plan, exported as ggufb200_linear_plan).
+"""Host arithmetic of the fused Linear's tiling (csrc/linear_sm90.cu::mma_splits for
+GGUFB200_ALGO_FUSED_MMA, exported as ggufb200_linear_plan).
 
 A wrong plan is the kind of bug that HANGS a GPU (a K range with no k-blocks never signals its barriers), so the invariants
 are checked here on the CPU over many shapes: every K range owns whole 256-wide spans, none is empty, together they cover K
@@ -80,7 +81,7 @@ def test_nosplit_flag_disables_every_split(pkg):
         assert L.ggufb200_linear_workspace(int(Q.Q4_K), M, N, K, 1, FUSED_TMEM | NOSPLIT) == 0
 
 
-# ---------------------------------------------------------------- FUSED_TMEM kernel (csrc/gemm4.cu::g4_plan)
+# ---------------------------------------------------------------- FUSED_TMEM kernel (csrc/linear_sm90.cu::tmem_plan)
 def _check_tmem(L, M, N, K, ws, flags=0):
     rc, (tokens, ranges, kb, items) = _plan(L, Q.Q4_K, M, N, K, ws, FUSED_TMEM | flags)
     assert rc == 0

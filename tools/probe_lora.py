@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One (M, N, K) Q4_K Linear with a rank-R LoRA patch: in-kernel (extra k-block of gemm4) vs side GEMMs -- difference and time.
+"""One (M, N, K) Q4_K Linear with a rank-R LoRA patch: in-kernel (extra k-block of FUSED_TMEM) vs side GEMMs -- difference and time.
 Run one shape per process under `timeout` so a hang is contained:  python tools/probe_lora.py M N K [rank]"""
 import os
 import sys
