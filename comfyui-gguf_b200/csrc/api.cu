@@ -215,15 +215,9 @@ size_t ggufb200_linear_workspace(int ggml_type, int64_t M, int64_t N, int64_t K,
     return ggufb200_linear_workspace_ex(ggml_type, M, N, K, act_dtype, kF16, algo);
 }
 
-struct LoraSide {
-    const void *T;      // [M, 64] activation dtype: x * down^T, zero padded beyond the rank
-    int64_t ldt;
-    const void *U;      // [N, 64] fp16: scale * up, zero padded
-};
-
 static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans, int64_t N, int64_t K, const void *X, int64_t M, int64_t ldx,
                        int act_dtype, int math_dtype, const void *bias, int bias_dtype, void *Y, int64_t ldy, void *workspace,
-                       size_t workspace_bytes, int algo, void *stream, const LoraSide *lora = nullptr)
+                       size_t workspace_bytes, int algo, void *stream, const LoraOperands *lora = nullptr)
 {
     int bs, ts;
     if (!type_geom(ggml_type, &bs, &ts)) return GGUFB200_E_TYPE;
@@ -251,10 +245,14 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
     if (!aligned16(X) || (ldx % 8) != 0) return GGUFB200_E_ALIGN;
     if (vec_y && (!aligned16(Y) || (ldy % 8) != 0)) return GGUFB200_E_ALIGN;
     if (workspace && !aligned16(workspace) && r.ws) return GGUFB200_E_ALIGN;
-    if (lora) {     // the rank-r update rides as one extra k-block of the FUSED_TMEM kernel: no other route can carry it
+    if (lora) {     // the rank-r update rides as J extra k-blocks of the FUSED_TMEM kernel: no other route can carry it
+        if (lora->kblocks < 1 || lora->kblocks > kLoraMaxKblocks) return GGUFB200_E_SHAPE;
         if (r.algo != GGUFB200_ALGO_FUSED_TMEM) return GGUFB200_E_UNSUPPORTED;
         if (!lora->T || !lora->U) return GGUFB200_E_NULL;
-        if (!aligned16(lora->T) || !aligned16(lora->U) || lora->ldt < 64 || (lora->ldt % 8) != 0) return GGUFB200_E_ALIGN;
+        const long long width = 64ll * lora->kblocks;
+        if (!aligned16(lora->T) || !aligned16(lora->U) || lora->ldt < width || (lora->ldt % 8) != 0 || lora->ldu < width || (lora->ldu % 8) != 0 ||
+            (reinterpret_cast<uintptr_t>(lora->tiles) & 3))
+            return GGUFB200_E_ALIGN;
     }
     if (int rc = device_check()) return rc;
     cudaStream_t st = (cudaStream_t)stream;
@@ -273,7 +271,7 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
         long long span_stride = 0;
         if (W_spans) repack_bytes(ggml_type, N, K, nullptr, &span_stride);
         return fused_tmem_linear(ggml_type, W_packed, W_spans, span_stride, N, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, workspace,
-                                 ws_avail, opt, lora ? lora->T : nullptr, lora ? lora->ldt : 0, lora ? lora->U : nullptr, st);
+                                 ws_avail, opt, lora ? *lora : LoraOperands{}, st);
     }
     case GGUFB200_ALGO_DEQUANT_MMA: {
         if (ws_avail < dense) return GGUFB200_E_WORKSPACE;
@@ -305,9 +303,18 @@ int ggufb200_linear_lora(int ggml_type, const void *W_packed, const void *W_span
                          int act_dtype, const void *bias, int bias_dtype, const void *T, int64_t ldt, const void *U, void *Y, int64_t ldy,
                          void *workspace, size_t workspace_bytes, int algo, void *stream)
 {
-    const LoraSide side{T, ldt, U};
+    return ggufb200_linear_lora_ex(ggml_type, W_packed, W_spans, N, K, X, M, ldx, act_dtype, bias, bias_dtype, T, ldt, U, 64, 1, nullptr, Y, ldy,
+                                   workspace, workspace_bytes, algo, stream);
+}
+
+int ggufb200_linear_lora_ex(int ggml_type, const void *W_packed, const void *W_spans, int64_t N, int64_t K, const void *X, int64_t M, int64_t ldx,
+                            int act_dtype, const void *bias, int bias_dtype, const void *T, int64_t ldt, const void *U, int64_t ldu,
+                            int lora_kblocks, const int32_t *tile_kblocks, void *Y, int64_t ldy, void *workspace, size_t workspace_bytes, int algo,
+                            void *stream)
+{
+    const LoraOperands lora{T, ldt, U, ldu, lora_kblocks, tile_kblocks};
     return linear_impl(ggml_type, W_packed, W_spans, N, K, X, M, ldx, act_dtype, kF16, bias, bias_dtype, Y, ldy, workspace, workspace_bytes, algo,
-                       stream, &side);
+                       stream, &lora);
 }
 
 size_t ggufb200_repack_bytes(int ggml_type, int64_t N, int64_t K)

@@ -51,13 +51,22 @@ void fused_mma_plan(long long M, long long N, long long K, size_t ws_bytes, cons
 int fused_mma_linear(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype,
                      const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes, const LinearOptions &opt,
                      cudaStream_t st);
-// GGUFB200_ALGO_FUSED_TMEM: the transposed product, token tiles sized to the activation, optional LoRA k-block.
+// GGUFB200_ALGO_FUSED_TMEM: the transposed product, token tiles sized to the activation, optional LoRA k-blocks.
+constexpr int kLoraMaxKblocks = 8;
+struct LoraOperands {
+    const void *T;         // x * down^T: [M, 64 * kblocks] activation dtype, row stride ldt; nullptr = no LoRA
+    long long ldt;
+    const void *U;         // scale * up: [N, 64 * kblocks] fp16, row stride ldu
+    long long ldu;
+    int kblocks;           // J, 1 .. kLoraMaxKblocks
+    const int32_t *tiles;  // (first, count) per 128-feature tile, ceil(N / 128) pairs, or nullptr = every tile runs all J
+};
 bool fused_tmem_supported(int type, const void *W, long long N, long long K);
 size_t fused_tmem_workspace(long long M, long long N, long long K, const LinearOptions &opt);
 void fused_tmem_plan(long long M, long long N, long long K, size_t ws_bytes, const LinearOptions &opt, int *tile_tokens, int *splits,
                      int *spans_per_split, int *items);
 int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
                       long long ldx, int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes,
-                      const LinearOptions &opt, const void *loraT, long long ldt, const void *loraU, cudaStream_t st);
+                      const LinearOptions &opt, const LoraOperands &lora, cudaStream_t st);
 
 }  // namespace ggufb200

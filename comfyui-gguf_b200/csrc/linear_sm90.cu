@@ -17,8 +17,10 @@
 //                       the row stride are multiples of 16 bytes) or from the span-major copy of repack.cu (every format).
 //                       With bf16 activations the weight is cast to bf16 (the reference's cast before F.linear).  Work item =
 //                       (K range, 256-feature tile, token tile), served by 2 * ACCS CTAs (128 features x TT tokens each).  An
-//                       optional LoRA update rides as one extra k-block of the K range 0: A = U rows (scale * up), B = T =
-//                       x * down^T.  K is processed in whole 256-wide spans: k-blocks past K are zero on both operands.
+//                       optional LoRA update rides as J <= 8 extra k-blocks of the K range 0: A = U rows (scale * up), B = T =
+//                       x * down^T, k-block j at columns 64 j of both; a per-tile table can narrow each 128-feature tile to the
+//                       k-blocks whose U rows are not zero there.  K is processed in whole 256-wide spans: k-blocks past K are
+//                       zero on both operands.
 //
 // Split-K (both fused routes): when the output tiles leave SMs idle, K is cut into ranges of whole 256-wide spans, one CTA
 // per (tile, range); each CTA stores its fp32 partial tile into its own slice of the caller's workspace ([S, M, N] fp32) and
@@ -255,9 +257,7 @@ struct TmemArgs {
     void *ws;
     size_t ws_bytes;
     const LinearOptions &opt;
-    const void *loraT;         // LoRA: T = x * down^T, [M, 64] activation dtype, row stride ldt (nullptr: none)
-    long long ldt;
-    const void *loraU;         // LoRA: U = scale * up, fp16 [N, 64] contiguous
+    const LoraOperands &lora;  // lora.T == nullptr: no LoRA k-blocks
     cudaStream_t st;
 };
 
@@ -267,7 +267,7 @@ static int tmem_launch(const TmemArgs &a, const TmemPlan &pl, float *partial)
     CUtensorMap tmX, tmT;
     if (!make_kblock_map(&tmX, a.X, a.M, a.K, a.ldx, ACT, TT)) return GGUFB200_E_CUDA;
     tmT = tmX;
-    if (a.loraT && !make_kblock_map(&tmT, a.loraT, a.M, 64, a.ldt, ACT, TT)) return GGUFB200_E_CUDA;
+    if (a.lora.T && !make_kblock_map(&tmT, a.lora.T, a.M, (long long)kBlockK * a.lora.kblocks, a.lora.ldt, ACT, TT)) return GGUFB200_E_CUDA;
     WgParams p{};
     p.M = a.M; p.N = a.N; p.K = a.K;
     p.bias = partial ? nullptr : a.bias;
@@ -279,7 +279,10 @@ static int tmem_launch(const TmemArgs &a, const TmemPlan &pl, float *partial)
     p.row_bytes = a.K / Q::BS * Q::TS;
     p.Wspan = reinterpret_cast<const uint8_t *>(a.Wspan);
     p.span_stride = a.span_stride;
-    p.loraU = a.loraT ? reinterpret_cast<const uint16_t *>(a.loraU) : nullptr;
+    p.loraU = a.lora.T ? reinterpret_cast<const uint16_t *>(a.lora.U) : nullptr;
+    p.ldu = a.lora.ldu;
+    p.lora_kb = a.lora.kblocks;
+    p.lora_tiles = a.lora.tiles;
     p.ftiles = 2 * pl.ftiles;                        // 128-feature halves of the 256-feature item
     p.ttiles = pl.ttiles * pl.accs;                  // TT-token parts of the TT * ACCS-token item
     p.kb_per_split = 4 * pl.spans_per_split;
@@ -336,10 +339,10 @@ bool fused_tmem_supported(int type, const void *W, long long N, long long K)
 
 int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
                       long long ldx, int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes,
-                      const LinearOptions &opt, const void *loraT, long long ldt, const void *loraU, cudaStream_t st)
+                      const LinearOptions &opt, const LoraOperands &lora, cudaStream_t st)
 {
     if (N % 8 != 0 || K % 8 != 0) return GGUFB200_E_UNSUPPORTED;
-    const TmemArgs a{W, Wspan, span_stride, N, K, X, M, ldx, bias, bias_dtype, Y, ldy, ws, ws_bytes, opt, loraT, ldt, loraU, st};
+    const TmemArgs a{W, Wspan, span_stride, N, K, X, M, ldx, bias, bias_dtype, Y, ldy, ws, ws_bytes, opt, lora, st};
     return with_block(type, GGUFB200_E_UNSUPPORTED, [&](auto blk) {
         using Q = decltype(blk);
         if (!Wspan && !canonical_ok<Q>(W, K)) return GGUFB200_E_UNSUPPORTED;

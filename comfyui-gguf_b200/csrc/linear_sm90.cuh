@@ -34,9 +34,12 @@ struct WgParams {
     long long row_bytes;
     const uint8_t *Wspan;    // span-major copy (repack.cu) or nullptr
     long long span_stride;   // bytes between consecutive spans of the span-major copy
-    const uint16_t *loraU;   // fp16 [N, 64] = scale * up: one extra k-block on the K range 0 (TRANS only)
+    const uint16_t *loraU;   // fp16 [N, ldu] = scale * up: lora_kb extra k-blocks on the K range 0 (TRANS only)
     int ttiles, ftiles;      // output tiles along tokens / features; CTA = (split, ftile, ttile), token tile fastest
     int kb_per_split, kb_total;
+    long long ldu;
+    int lora_kb;             // LoRA k-blocks: T columns / U columns 64 j .. 64 j + 63, j < lora_kb
+    const int *lora_tiles;   // per 128-feature tile (first, count): the LoRA k-blocks that tile runs; nullptr = all lora_kb
 };
 
 template <int TN, bool TRANS> struct WgCfg {
@@ -82,8 +85,17 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     if (tok0 >= p.M || feat0 >= p.N) return;                 // tile of the plan past the edge (uniform over the CTA)
     const int kb0 = split * p.kb_per_split;
     const int nkb_main = min(p.kb_per_split, p.kb_total - kb0);
-    const bool lora = p.loraU != nullptr && split == 0;
-    const int nkb = nkb_main + (lora ? 1 : 0);
+    // LoRA k-blocks lora_first .. lora_first + lora_n - 1 follow the main loop; producer and consumers read the same pair
+    int lora_first = 0, lora_n = 0;
+    if (p.loraU != nullptr && split == 0) {
+        lora_n = p.lora_kb;
+        if (p.lora_tiles) {
+            const long long ft = feat0 / 128;
+            lora_first = min(max(p.lora_tiles[2 * ft], 0), p.lora_kb);
+            lora_n = min(max(p.lora_tiles[2 * ft + 1], 0), p.lora_kb - lora_first);
+        }
+    }
+    const int nkb = nkb_main + lora_n;
 
     extern __shared__ uint8_t wg_smem_raw[];
     uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(wg_smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -111,10 +123,11 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
             uint8_t *x_tile = TRANS ? b_tile : a_tile;
             uint8_t *w_tile = TRANS ? a_tile : b_tile;
             const int kb = kb0 + i;
-            const bool lora_kb = i == nkb_main;                // the extra k-block: X -> T = x * down^T, W -> U = scale * up
+            const bool lora_kb = i >= nkb_main;                // LoRA k-block lj: X -> T = x * down^T, W -> U = scale * up
+            const int lj = lora_first + i - nkb_main;
             if (t == 0) {
                 mbar_arrive_expect_tx(&full[s], TOK * 128 + (DENSE ? WROWS * 128 : 0));
-                tma_load_2d(x_tile, lora_kb ? &tmT : &tmX, &full[s], lora_kb ? 0 : kb * kBlockK, (int)tok0);
+                tma_load_2d(x_tile, lora_kb ? &tmT : &tmX, &full[s], lora_kb ? lj * kBlockK : kb * kBlockK, (int)tok0);
                 if constexpr (DENSE) tma_load_2d(w_tile, &tmW, &full[s], kb * kBlockK, (int)feat0);
             }
             if constexpr (!DENSE) {
@@ -134,7 +147,7 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
 #pragma unroll
                         for (int c = 0; c < 8; ++c) st_shared_v4(dst + (uint32_t)(c << 4), 0, 0, 0, 0);
                     } else if (lora_kb) {
-                        const uint4 *urow = reinterpret_cast<const uint4 *>(p.loraU + n * 64);
+                        const uint4 *urow = reinterpret_cast<const uint4 *>(p.loraU + n * p.ldu + lj * kBlockK);
 #pragma unroll
                         for (int half = 0; half < 2; ++half) {
                             uint32_t o[16];

@@ -143,7 +143,8 @@ def span_layout(weight, wraw):
     return out
 
 
-LORA_MAX_RANK = 64     # the LoRA k-block of the FUSED_TMEM kernel is one 64-wide k-block
+LORA_MAX_RANK = 64     # width of one LoRA k-block of the FUSED_TMEM kernel
+LORA_KERNEL_MAX_RANK = 8 * LORA_MAX_RANK     # at most 8 LoRA k-blocks: a larger total rank takes the side GEMMs (`_add_lora`)
 
 
 def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None):
@@ -177,12 +178,20 @@ def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None
         ws_ptr = ws.data_ptr()
     index = device.index
     if lora is not None:
-        t_pad, u_pad = lora           # T = x * down^T [M, 64] act dtype, U = scale * up [N, 64] fp16 (zero padded)
-
-        def call():
-            return L.ggufb200_linear_lora(qcode, w_ptr, None if spans is None else spans.data_ptr(), N, K, x2.data_ptr(), M, x2.stride(0), act,
-                                          bias_ptr, bias_code, t_pad.data_ptr(), t_pad.stride(0), u_pad.data_ptr(), y.data_ptr(), N, ws_ptr, need,
-                                          algo, _current_stream_ptr(index))
+        # T = x * down^T [M, 64 J] act dtype, U = scale * up [N, 64 J] fp16 (zero padded), per-tile k-block ranges or None
+        t_pad, u_pad, tiles = lora
+        J = u_pad.shape[1] // LORA_MAX_RANK
+        if J == 1 and tiles is None:
+            def call():
+                return L.ggufb200_linear_lora(qcode, w_ptr, None if spans is None else spans.data_ptr(), N, K, x2.data_ptr(), M, x2.stride(0), act,
+                                              bias_ptr, bias_code, t_pad.data_ptr(), t_pad.stride(0), u_pad.data_ptr(), y.data_ptr(), N, ws_ptr,
+                                              need, algo, _current_stream_ptr(index))
+        else:
+            def call():
+                return L.ggufb200_linear_lora_ex(qcode, w_ptr, None if spans is None else spans.data_ptr(), N, K, x2.data_ptr(), M, x2.stride(0),
+                                                 act, bias_ptr, bias_code, t_pad.data_ptr(), t_pad.stride(0), u_pad.data_ptr(), u_pad.stride(0), J,
+                                                 None if tiles is None else tiles.data_ptr(), y.data_ptr(), N, ws_ptr, need, algo,
+                                                 _current_stream_ptr(index))
     elif spans is not None:
         def call():
             return L.ggufb200_linear_spans(qcode, w_ptr, spans.data_ptr(), N, K, x2.data_ptr(), M, x2.stride(0), act, math, bias_ptr, bias_code,
@@ -258,10 +267,29 @@ def lora_side_terms(patches):
     reshape))` or a LoRAAdapter object carrying the same tuple in `.weights`.  Returns [(scale, up[N, r], down[r, K]), ...]
     with scale = strength_patch * alpha / r, or None when any entry needs the general `calculate_weight` machinery
     (strength_model != 1, offset / function hooks, LoCon mid weights, DoRA, reshape, diff / loha / lokr ... patches)."""
+    terms = lora_band_terms(patches)
+    if terms is None or any(band is not None for _s, _u, _d, band in terms):
+        return None
+    return [(scale, up, down) for scale, up, down, _band in terms]
+
+
+def lora_band_terms(patches):
+    """`lora_side_terms` that also accepts an `offset = (dim, start, size)`: the LoRA patches the band `start .. start + size`
+    of the output rows (dim 0) or of the input features (dim 1) only.  ComfyUI gives diffusers-format LoRAs such offsets, one
+    entry per q / k / v / mlp slice of a fused Flux or SD3 weight.  Returns [(scale, up, down, band), ...] with band None
+    (the whole weight) or (dim, start, size), or None when any entry needs `calculate_weight` (as `lora_side_terms`)."""
     terms = []
     for entry in patches:
-        if len(entry) < 3 or entry[2] != 1.0 or any(extra is not None for extra in entry[3:5]):
+        if len(entry) < 3 or entry[2] != 1.0 or (len(entry) > 4 and entry[4] is not None):
             return None
+        offset = entry[3] if len(entry) > 3 else None
+        band = None
+        if offset is not None:
+            if not isinstance(offset, (tuple, list)) or len(offset) != 3 or offset[0] not in (0, 1):
+                return None
+            band = (int(offset[0]), int(offset[1]), int(offset[2]))
+            if band[1] < 0 or band[2] <= 0:
+                return None
         value = entry[1]
         if type(value).__name__ == "LoRAAdapter" and hasattr(value, "weights"):
             payload = value.weights
@@ -276,8 +304,45 @@ def lora_side_terms(patches):
         if not (torch.is_tensor(up) and torch.is_tensor(down)) or up.dim() != 2 or down.dim() != 2 or up.shape[1] != down.shape[0]:
             return None
         scale = float(entry[0]) * (1.0 if alpha is None else float(alpha) / down.shape[0])
-        terms.append((scale, up, down))
+        terms.append((scale, up, down, band))
     return terms
+
+
+def lora_kernel_operands(terms, N, K, dtype, device):
+    """Pack recognised LoRA terms ([(scale, up, down, band), ...], shapes checked) into the operands of
+    ggufb200_linear_lora_ex: down_pad [64 J, K] in `dtype`, U [N, 64 J] fp16 = scale * up, and the per-tile k-block table
+    (int32 [ceil(N / 128), 2] of (first, count), or None when no term has a band).  A term takes the next r columns; its up
+    rows land on its output band (zero elsewhere), its down columns on its input band.  Terms are ordered by output band, so
+    the columns a 128-feature tile needs are contiguous and few: with disjoint q / k / v bands a tile runs only the k-blocks
+    of the bands it overlaps."""
+    def rows(band):
+        return (band[1], band[1] + band[2]) if band is not None and band[0] == 0 else (0, N)
+
+    order = sorted(terms, key=lambda t: rows(t[3]))
+    R = sum(down.shape[0] for _s, _u, down, _b in order)
+    J = max(1, -(-R // LORA_MAX_RANK))
+    down_pad = torch.zeros(J * LORA_MAX_RANK, K, device=device, dtype=dtype)
+    u_pad = torch.zeros(N, J * LORA_MAX_RANK, device=device, dtype=torch.float16)
+    n_tiles = -(-N // 128)
+    lo, hi = [None] * n_tiles, [None] * n_tiles            # column range per 128-feature tile
+    r0 = 0
+    for scale, up, down, band in order:
+        r = down.shape[0]
+        n0, n1 = rows(band)
+        k0, k1 = (band[1], band[1] + band[2]) if band is not None and band[0] == 1 else (0, K)
+        down_pad[r0:r0 + r, k0:k1] = down.to(device=device, dtype=dtype)
+        u_pad[n0:n1, r0:r0 + r] = (up.to(device=device, dtype=torch.float32) * scale).to(torch.float16)
+        if r:
+            for tile in range(n0 // 128, -(-n1 // 128)):
+                lo[tile] = r0 if lo[tile] is None else min(lo[tile], r0)
+                hi[tile] = r0 + r if hi[tile] is None else max(hi[tile], r0 + r)
+        r0 += r
+    tiles = None
+    if any(band is not None for *_t, band in terms):
+        pairs = [(0, 0) if lo[i] is None else (lo[i] // LORA_MAX_RANK, (hi[i] - 1) // LORA_MAX_RANK - lo[i] // LORA_MAX_RANK + 1)
+                 for i in range(n_tiles)]
+        tiles = torch.tensor(pairs, dtype=torch.int32).to(device)
+    return down_pad, u_pad, tiles
 
 
 class GGMLLayer(torch.nn.Module):
@@ -426,50 +491,58 @@ class GGMLOps(comfy_ops.manual_cast):
             entries = []
             for patch_list, _key in w.patches:
                 entries.extend(patch_list)
-            terms = lora_side_terms(entries)
+            terms = lora_band_terms(entries)
             if terms is None:
                 return None
             N, K = tuple(w.tensor_shape)
-            if any(tuple(up.shape) != (N, down.shape[0]) or down.shape[1] != K for _s, up, down in terms):
-                return None
+            for _s, up, down, band in terms:
+                rows, cols = N, K
+                if band is not None:
+                    dim, start, size = band
+                    if start + size > (N, K)[dim]:
+                        return None
+                    rows, cols = (size, K) if dim == 0 else (N, size)
+                if tuple(up.shape) != (rows, down.shape[0]) or down.shape[1] != cols:
+                    return None
             return terms
 
-        # LoRA inside the fused kernel (GGUFB200_ALGO_FUSED_TMEM, csrc/linear_sm90.cu: one extra k-block, SURVEY 8f rank 1):
-        # U = scale * up (fp16 [N, 64]) and down (act dtype [64, K]), zero padded to rank 64 and cached per patch set; per forward only T = x * down^T
-        # ([M, 64], this package's dense tensor-core GEMM) is computed before the fused call.
-        # False -> the unpatched fused kernel plus two library GEMMs of rank sum(r) (`_add_lora`).
+        # LoRA inside the fused kernel (GGUFB200_ALGO_FUSED_TMEM, csrc/linear_sm90.cu: J <= 8 extra k-blocks, SURVEY 8f rank 1):
+        # U = scale * up (fp16 [N, 64 J]), down (act dtype [64 J, K]) and, for row-band patches, the per-tile k-block table are
+        # cached per patch set (`lora_kernel_operands`); per forward only T = x * down^T ([M, 64 J], this package's dense
+        # tensor-core GEMM) is computed before the fused call.
+        # False -> the unpatched fused kernel plus library GEMMs of rank sum(r) (`_add_lora`), as for sum(r) > 512.
         lora_in_kernel = True
 
         def _lora_operands(self, terms, dev, dtype):
             # identity + storage + version of every factor: a patch set that was swapped for another one (even at a recycled
             # id()) or modified in place rebuilds the operands
-            key = tuple((id(up), up.data_ptr(), up._version, tuple(up.shape), id(down), down.data_ptr(), down._version, float(scale))
-                        for scale, up, down in terms) + (str(dev), dtype)
+            key = tuple((id(up), up.data_ptr(), up._version, tuple(up.shape), id(down), down.data_ptr(), down._version, float(scale), band)
+                        for scale, up, down, band in terms) + (str(dev), dtype)
             cached = self.__dict__.get("_gg_lora")
             if cached is not None and cached[0] == key:
-                return cached[1], cached[2]
+                return cached[1]
             N, K = tuple(self.weight.tensor_shape)
-            down_pad = torch.zeros(LORA_MAX_RANK, K, device=dev, dtype=dtype)
-            u_pad = torch.zeros(N, LORA_MAX_RANK, device=dev, dtype=torch.float16)
-            r0 = 0
-            for scale, up, down in terms:
-                r = down.shape[0]
-                down_pad[r0:r0 + r] = down.to(device=dev, dtype=dtype)
-                u_pad[:, r0:r0 + r] = (up.to(device=dev, dtype=torch.float32) * scale).to(torch.float16)
-                r0 += r
-            self.__dict__["_gg_lora"] = (key, down_pad, u_pad)
-            return down_pad, u_pad
+            operands = lora_kernel_operands(terms, N, K, dtype, dev)
+            self.__dict__["_gg_lora"] = (key, operands)
+            return operands
 
         def _add_lora(self, y, input, terms):
             x2 = input.reshape(-1, input.shape[-1])
             y2 = y.view(-1, y.shape[-1])
+            if any(band is not None for *_t, band in terms):     # one pair of GEMMs per term, on its bands of x and y
+                for scale, up, down, band in terms:
+                    xs = x2[:, band[1]:band[1] + band[2]] if band is not None and band[0] == 1 else x2
+                    ys = y2[:, band[1]:band[1] + band[2]] if band is not None and band[0] == 0 else y2
+                    t = xs @ down.to(device=x2.device, dtype=x2.dtype, non_blocking=True).t()
+                    ys.addmm_(t, (up.to(device=x2.device, dtype=torch.float32, non_blocking=True) * scale).to(x2.dtype).t())
+                return y
             if len(terms) == 1:
-                scale, up, down = terms[0]
+                scale, up, down, _band = terms[0]
                 down_all = down.to(device=x2.device, dtype=x2.dtype, non_blocking=True)
                 up_all = up.to(device=x2.device, dtype=torch.float32, non_blocking=True) * scale
             else:                                                   # one pair of GEMMs for any number of LoRAs
-                down_all = torch.cat([d.to(device=x2.device, dtype=x2.dtype, non_blocking=True) for _s, _u, d in terms], 0)
-                up_all = torch.cat([u.to(device=x2.device, dtype=torch.float32, non_blocking=True) * s for s, u, _d in terms], 1)
+                down_all = torch.cat([d.to(device=x2.device, dtype=x2.dtype, non_blocking=True) for _s, _u, d, _b in terms], 0)
+                up_all = torch.cat([u.to(device=x2.device, dtype=torch.float32, non_blocking=True) * s for s, u, _d, _b in terms], 1)
             t = x2 @ down_all.t()                                   # [M, R]   library GEMMs: R is tens, not thousands
             y2.addmm_(t, up_all.to(x2.dtype).t())
             return y
@@ -508,10 +581,10 @@ class GGMLOps(comfy_ops.manual_cast):
                         algo = _lib.ALGO_FUSED_TMEM | exact
                     lora = None
                     if (terms and self.lora_in_kernel and math == _F16_CODE and N % 8 == 0
-                            and qtype != _Q.BF16 and sum(d.shape[0] for _s, _u, d in terms) <= LORA_MAX_RANK
+                            and qtype != _Q.BF16 and sum(d.shape[0] for _s, _u, d, _b in terms) <= LORA_KERNEL_MAX_RANK
                             and (spans is not None or not needs_span_layout(qtype, K))):
-                        down_pad, u_pad = self._lora_operands(terms, dev, input.dtype)
-                        lora = (linear_dense(input.reshape(-1, K), down_pad), u_pad)       # T = x * down^T, [M, 64]
+                        down_pad, u_pad, tiles = self._lora_operands(terms, dev, input.dtype)
+                        lora = (linear_dense(input.reshape(-1, K), down_pad), u_pad, tiles)       # T = x * down^T, [M, 64 J]
                         algo = _lib.ALGO_FUSED_TMEM | exact
                     y = _launch_linear(input, wraw, qtype, N, K, b, math, algo, spans, lora)
                     if lora is not None:

@@ -205,6 +205,22 @@ int ggufb200_linear_lora(int ggml_type, const void *W_packed, const void *W_span
                          void *Y, int64_t ldy, void *workspace, size_t workspace_bytes, int algo, void *stream);
 
 /*
+ * ggufb200_linear_lora with a total rank up to 512 and per-tile LoRA ranges (row-band patches such as diffusers-format
+ * LoRAs on fused qkv weights):
+ *     Y = X * dequant(W)^T + T * U^T (+ bias),   T [M, 64*J] act_dtype (row stride ldt),   U [N, 64*J] fp16 (row stride ldu)
+ * The update is J = lora_kblocks extra 64-wide k-blocks (1 <= J <= 8, else GGUFB200_E_SHAPE); k-block j reads columns
+ * 64*j .. 64*j+63 of T and U.  ldt and ldu must be at least 64*J and multiples of 8 (GGUFB200_E_ALIGN).
+ * tile_kblocks (device memory, may be NULL): ceil(N / 128) pairs of int32 (first, count), one pair per 128 output features
+ * n = 128*i .. 128*i+127; those features add only k-blocks first .. first+count-1 (count = 0: none; values are clamped to
+ * 0 .. J).  Columns of U that are zero on a tile's rows may be skipped this way without changing the result.  NULL: every
+ * tile adds all J k-blocks.  ggufb200_linear_lora is this call with ldu = 64, J = 1, tile_kblocks = NULL.
+ */
+int ggufb200_linear_lora_ex(int ggml_type, const void *W_packed, const void *W_spans, int64_t N, int64_t K, const void *X, int64_t M,
+                            int64_t ldx, int act_dtype, const void *bias, int bias_dtype, const void *T, int64_t ldt, const void *U,
+                            int64_t ldu, int lora_kblocks, const int32_t *tile_kblocks, void *Y, int64_t ldy, void *workspace,
+                            size_t workspace_bytes, int algo, void *stream);
+
+/*
  * Plain tensor-core GEMM on an already-dense weight: Y = X * W^T (+bias), W[N,K] in
  * act_dtype.  Used for the F16/BF16 (torch-compatible) Linears of a model and as the
  * second half of GGUFB200_ALGO_DEQUANT_MMA.

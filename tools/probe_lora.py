@@ -51,7 +51,7 @@ with torch.no_grad():
         torch.cuda.synchronize()
         res[mode] = (y, gpu_us(lambda: lin(x)))
     terms = lin._lora_terms(dev)
-    down_pad, u_pad = lin._lora_operands(terms, dev, x.dtype)
+    down_pad, _u_pad, _tiles = lin._lora_operands(terms, dev, x.dtype)
     t_gemm = gpu_us(lambda: ops.linear_dense(x, down_pad))
     lin.weight.patches = []
     plain = gpu_us(lambda: lin(x))
