@@ -57,21 +57,22 @@ struct Route {
     size_t ws;         // workspace bytes the route wants (0 = none)
 };
 
-// GGUFB200_FLAG_* bits -> the options of the warpgroup-MMA routes (GENERIC wins over EXACT_W, TILE384 over TILE192)
-static LinearOptions linear_options(int flags)
+// GGUFB200_FLAG_* bits -> the options of the warpgroup-MMA routes (GENERIC wins over EXACT_W, TILE384 over TILE192).
+// A straddled weight never cuts K into ranges.
+static LinearOptions linear_options(int flags, bool straddled)
 {
     LinearOptions o;
     if (flags & GGUFB200_FLAG_GENERIC) o.producers = LinearOptions::GENERIC;
     else if (flags & GGUFB200_FLAG_EXACT_W) o.producers = LinearOptions::EXACT;
     if (flags & GGUFB200_FLAG_TILE384) o.tile = 384;
     else if (flags & GGUFB200_FLAG_TILE192) o.tile = 192;
-    o.nosplit = (flags & GGUFB200_FLAG_NOSPLIT) != 0;
+    o.nosplit = (flags & GGUFB200_FLAG_NOSPLIT) != 0 || straddled;
     return o;
 }
 
 // `W` may be NULL (workspace query: assume a 16-byte aligned weight); ws_avail = workspace the caller supplied (SIZE_MAX in a query);
 // have_spans: the caller also holds the re-packed span-major copy of the weight (ggufb200_repack), which the FUSED_TMEM
-// kernel can read for every block format and every K
+// kernel can read for every block format and every K (for a straddled weight: the block-major copy)
 static Route pick_route(int type, const void *W, long long M, long long N, long long K, int act, int math, int algo_flags,
                         const LinearOptions &opt, size_t ws_avail, bool have_spans = false)
 {
@@ -79,7 +80,10 @@ static Route pick_route(int type, const void *W, long long M, long long N, long 
     const int flags = algo_flags & ~GGUFB200_ALGO_MASK;
     const size_t dense = (size_t)N * (size_t)K * 2;
     const bool w_ok = !W || aligned16(W);
-    const bool fusable = fused_type(type) && math == kF16 && (K % 64) == 0 && (N % 8) == 0;
+    int bs = 1;
+    type_geom(type, &bs, nullptr);
+    const bool straddled = straddled_rows(bs, N, K);
+    const bool fusable = fused_type(type) && math == kF16 && (K % 64) == 0 && (N % 8) == 0 && !straddled;
     Route r{algo, 0};
     if (algo == GGUFB200_ALGO_AUTO) {
         // Measured on an H100 80GB HBM3 (400 W power limit, Q4_K / Q6_K at Flux shapes, tools/bench_linear.py --graph):
@@ -89,10 +93,15 @@ static Route pick_route(int type, const void *W, long long M, long long N, long 
         //  * weights that kernel cannot read (no span-major copy at hand): dequant once + the dense GEMM took 0.18-0.89 of the
         //    fused reference-exact kernel's time at every M from 64 to 4608, so FUSED_MMA is only taken when the caller's
         //    workspace cannot hold the dequantised weight.
+        //  * a straddled weight (SD1.5 / SDXL K-quants at K % 256 != 0): dequant + dense GEMM at every M.  The GEMVs index whole rows;
+        //    above M = 8, tools/bench_sd_linears.py (bf16 and fp16, Q4_K / Q6_K, M = 256 .. 8192, (N, K) = (640, 640), (5120, 640),
+        //    (320, 320), (2560, 320)) measured dequant + GEMM at 0.58-1.05 of the reference-exact FUSED_TMEM kernel's time, 0.58-0.93
+        //    for Q6_K (which FUSED_TMEM reads from the block-major copy).  FUSED_TMEM serves them when asked for (and the LoRA k-blocks).
         // A math dtype other than fp16 means the reference's own sequence in that dtype: standalone dequant + dense GEMM (or the GEMV).
         const bool tmem_ok = w_ok && fused_type(type) && math == kF16 && (N % 8) == 0 && (have_spans || fused_tmem_supported(type, W, N, K));
         const bool exact = (flags & GGUFB200_FLAG_EXACT_W) != 0 || math != kF16;
         if (!w_ok) r.algo = GGUFB200_ALGO_DEQUANT_MMA;
+        else if (straddled) r.algo = GGUFB200_ALGO_DEQUANT_MMA;
         else if (M <= gemv_max_m() && !exact && gemv2_supported(type, W ? W : (const void *)16, N, K, M)) r.algo = GGUFB200_ALGO_GEMV_FAST;
         else if (M <= gemv_max_m()) r.algo = GGUFB200_ALGO_GEMV;
         else if (tmem_ok) r.algo = GGUFB200_ALGO_FUSED_TMEM;
@@ -120,7 +129,7 @@ const char *ggufb200_strerror(int rc)
     case GGUFB200_E_TYPE: return "unsupported ggml quantization type (no CPU fallback is provided)";
     case GGUFB200_E_DTYPE: return "dtype code must be 0 (float16), 1 (bfloat16) or 2 (float32)";
     case GGUFB200_E_ALIGN: return "output / activation pointers must be 16-byte aligned";
-    case GGUFB200_E_SHAPE: return "bad shape: sizes must be non-negative, K a multiple of the block size, ld >= row length";
+    case GGUFB200_E_SHAPE: return "bad shape: sizes must be non-negative, K a multiple of the block size (or of 8 with N*K a multiple of a 256-element block), ld >= row length";
     case GGUFB200_E_NULL: return "required pointer is NULL";
     case GGUFB200_E_CUDA: return "CUDA launch failed";
     case GGUFB200_E_WORKSPACE: return "workspace too small (see ggufb200_linear_workspace)";
@@ -206,8 +215,9 @@ int ggufb200_dequant_rows(int ggml_type, const void *packed, int64_t n_table_row
 
 size_t ggufb200_linear_workspace_ex(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int math_dtype, int algo)
 {
-    if (!type_geom(ggml_type, nullptr, nullptr) || N <= 0 || K <= 0 || M <= 0) return 0;
-    return pick_route(ggml_type, nullptr, M, N, K, act_dtype, math_dtype, algo, linear_options(algo), (size_t)-1).ws;
+    int bs;
+    if (!type_geom(ggml_type, &bs, nullptr) || N <= 0 || K <= 0 || M <= 0) return 0;
+    return pick_route(ggml_type, nullptr, M, N, K, act_dtype, math_dtype, algo, linear_options(algo, straddled_rows(bs, N, K)), (size_t)-1).ws;
 }
 
 size_t ggufb200_linear_workspace(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int algo)
@@ -223,11 +233,14 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
     if (!type_geom(ggml_type, &bs, &ts)) return GGUFB200_E_TYPE;
     if (act_dtype != kF16 && act_dtype != kBF16) return GGUFB200_E_DTYPE;
     if (!dtype_ok(math_dtype) || (bias && !dtype_ok(bias_dtype))) return GGUFB200_E_DTYPE;
-    if (M < 0 || N <= 0 || K <= 0 || K % bs != 0 || K % 8 != 0 || ldx < K || ldy < N) return GGUFB200_E_SHAPE;
+    if (M < 0 || N <= 0 || K <= 0 || K % 8 != 0 || ldx < K || ldy < N) return GGUFB200_E_SHAPE;
+    // rows are whole blocks, or a straddled weight: the flat block stream of an [N, K] tensor (internal.h)
+    const bool straddled = straddled_rows(bs, N, K);
+    if (K % bs != 0 && !straddled) return GGUFB200_E_SHAPE;
     if (M == 0) return GGUFB200_OK;
     if (!W_packed || !X || !Y) return GGUFB200_E_NULL;
     const int flags = algo & ~GGUFB200_ALGO_MASK;
-    const LinearOptions opt = linear_options(flags);
+    const LinearOptions opt = linear_options(flags, straddled);
     const bool w_ok = aligned16(W_packed);
     const size_t dense = (size_t)N * (size_t)K * 2;
     const size_t ws_avail = (workspace && aligned16(workspace)) ? workspace_bytes : 0;
@@ -240,6 +253,8 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
     }
     if (W_spans && !aligned16(W_spans)) return GGUFB200_E_ALIGN;
     const Route r = pick_route(ggml_type, W_packed, M, N, K, act_dtype, math_dtype, algo, opt, ws_avail, W_spans != nullptr);
+    // the GEMVs and FUSED_MMA index whole rows of blocks: a straddled weight runs on FUSED_TMEM or dequant + GEMM only
+    if (straddled && r.algo != GGUFB200_ALGO_FUSED_TMEM && r.algo != GGUFB200_ALGO_DEQUANT_MMA) return GGUFB200_E_UNSUPPORTED;
     // the small-M kernel stores per element: it only needs 2-byte aligned Y rows; every other route moves 16-byte vectors
     const bool vec_y = r.algo != GGUFB200_ALGO_GEMV && r.algo != GGUFB200_ALGO_GEMV_FAST;
     if (!aligned16(X) || (ldx % 8) != 0) return GGUFB200_E_ALIGN;
@@ -275,7 +290,7 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
     }
     case GGUFB200_ALGO_DEQUANT_MMA: {
         if (ws_avail < dense) return GGUFB200_E_WORKSPACE;
-        int rc = dequant_dispatch(ggml_type, W_packed, N * (K / bs), workspace, act_dtype, math_dtype, st, (flags & GGUFB200_FLAG_W_STABLE) != 0);
+        int rc = dequant_dispatch(ggml_type, W_packed, N * K / bs, workspace, act_dtype, math_dtype, st, (flags & GGUFB200_FLAG_W_STABLE) != 0);
         if (rc != GGUFB200_OK) return rc;
         return dense_gemm(workspace, N, K, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st);
     }
@@ -320,7 +335,7 @@ int ggufb200_linear_lora_ex(int ggml_type, const void *W_packed, const void *W_s
 size_t ggufb200_repack_bytes(int ggml_type, int64_t N, int64_t K)
 {
     int bs;
-    if (!type_geom(ggml_type, &bs, nullptr) || N <= 0 || K <= 0 || K % bs != 0) return 0;
+    if (!type_geom(ggml_type, &bs, nullptr) || N <= 0 || K <= 0 || (K % bs != 0 && !straddled_rows(bs, N, K))) return 0;
     return repack_bytes(ggml_type, N, K, nullptr, nullptr);
 }
 
@@ -328,7 +343,7 @@ int ggufb200_repack(int ggml_type, const void *W_packed, int64_t N, int64_t K, v
 {
     int bs;
     if (!type_geom(ggml_type, &bs, nullptr) || ggml_type == T_BF16) return GGUFB200_E_TYPE;
-    if (N <= 0 || K <= 0 || K % bs != 0) return GGUFB200_E_SHAPE;
+    if (N <= 0 || K <= 0 || (K % bs != 0 && !straddled_rows(bs, N, K))) return GGUFB200_E_SHAPE;
     if (!W_packed || !out) return GGUFB200_E_NULL;
     if (!aligned16(out) || (reinterpret_cast<uintptr_t>(W_packed) & 1)) return GGUFB200_E_ALIGN;
     if (int rc = device_check()) return rc;
@@ -338,11 +353,12 @@ int ggufb200_repack(int ggml_type, const void *W_packed, int64_t N, int64_t K, v
 int ggufb200_linear_plan(int ggml_type, int64_t M, int64_t N, int64_t K, size_t workspace_bytes, int algo, int *tile_rows, int *k_ranges,
                          int *kblocks_per_range, int *ctas)
 {
-    if (!type_geom(ggml_type, nullptr, nullptr)) return GGUFB200_E_TYPE;
+    int bs;
+    if (!type_geom(ggml_type, &bs, nullptr)) return GGUFB200_E_TYPE;
     if (!tile_rows || !k_ranges || !kblocks_per_range || !ctas) return GGUFB200_E_NULL;
     if (M <= 0 || N <= 0 || K <= 0 || K % 64 != 0 || N % 8 != 0) return GGUFB200_E_SHAPE;
     if (!fused_type(ggml_type)) return GGUFB200_E_UNSUPPORTED;
-    const LinearOptions opt = linear_options(algo);
+    const LinearOptions opt = linear_options(algo, straddled_rows(bs, N, K));
     if ((algo & GGUFB200_ALGO_MASK) == GGUFB200_ALGO_FUSED_TMEM) {
         int spans = 1;
         fused_tmem_plan(M, N, K, workspace_bytes, opt, tile_rows, k_ranges, &spans, ctas);

@@ -26,7 +26,16 @@ bool gemv2_supported(int type, const void *W, long long N, long long K, long lon
 int gemv2_dispatch(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype, const void *bias,
                    int bias_dtype, void *Y, long long ldy, cudaStream_t st, bool w_stable = false);
 
+// A weight whose 256-element super-blocks straddle rows: the flat block stream of an [N, K] tensor with K % 256 != 0,
+// as the GGUF converter writes SD1.5 / SDXL K-quant tensors (reshaped to [N * K / 256, 256] before quantising).  Row n
+// starts at element n * K of the stream, which may fall inside a block.
+inline bool straddled_rows(int block_size, long long N, long long K)
+{
+    return block_size == 256 && K % 256 != 0 && (N * K) % 256 == 0;
+}
+
 // ------------------------------------------------------------------ repack.cu: the span-major copy of a packed weight
+// (block-major out[b][pitch] for a straddled weight: span_stride = pitch)
 size_t repack_bytes(int type, long long N, long long K, int *pitch, long long *span_stride);
 int repack_dispatch(int type, const void *W, long long N, long long K, void *out, cudaStream_t st);
 
@@ -37,7 +46,7 @@ struct LinearOptions {
     Producers producers = FAST;    // FUSED_TMEM weight producers: hand-written with one fused multiply-add per element (FAST),
                                    // hand-written with the reference's rounding sequence (EXACT), functor producers (GENERIC)
     int tile = 0;                  // FUSED_TMEM token items: 0 = the cost model picks, 192 or 384 = forced
-    bool nosplit = false;          // never cut K into ranges
+    bool nosplit = false;          // never cut K into ranges (always set for a straddled weight)
 };
 
 // `ws_bytes` is the usable workspace at `ws`: 0 when the caller passed none or a misaligned one.

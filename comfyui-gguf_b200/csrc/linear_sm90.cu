@@ -15,6 +15,10 @@
 //                       producers for the hot formats, the functor producer for the others), B = the TMA-fed activation tile.
 //                       The packed rows are read one 256-wide span at a time from the canonical layout (when a row's span and
 //                       the row stride are multiples of 16 bytes) or from the span-major copy of repack.cu (every format).
+//                       A straddled weight (straddled_rows(): SD1.5 / SDXL K-quants at K % 256 != 0) is read as the flat
+//                       stream of 256-element blocks it is, from the canonical bytes (Q4_K / Q5_K) or the block-major copy
+//                       of repack.cu (the others): k-block kb of row n is one quarter of block (n K + 64 kb) / 256, the
+//                       kernel runs K / 64 k-blocks and K is never split into ranges.
 //                       With bf16 activations the weight is cast to bf16 (the reference's cast before F.linear).  Work item =
 //                       (K range, 256-feature tile, token tile), served by 2 * ACCS CTAs (128 features x TT tokens each).  An
 //                       optional LoRA update rides as J <= 8 extra k-blocks of the K range 0: A = U rows (scale * up), B = T =
@@ -259,6 +263,7 @@ struct TmemArgs {
     const LinearOptions &opt;
     const LoraOperands &lora;  // lora.T == nullptr: no LoRA k-blocks
     cudaStream_t st;
+    bool straddled;            // straddled_rows(): W (or Wspan, the block-major copy) is a flat stream of 256-element blocks
 };
 
 template <class Q, class Prod, int ACT, int TT>
@@ -276,9 +281,14 @@ static int tmem_launch(const TmemArgs &a, const TmemPlan &pl, float *partial)
     p.ldy = a.ldy;
     p.partial = partial;
     p.W = reinterpret_cast<const uint8_t *>(a.W);
-    p.row_bytes = a.K / Q::BS * Q::TS;
-    p.Wspan = reinterpret_cast<const uint8_t *>(a.Wspan);
-    p.span_stride = a.span_stride;
+    if (a.straddled) {                               // the producers address blocks, not rows: base + block * stride
+        p.Wspan = reinterpret_cast<const uint8_t *>(a.Wspan ? a.Wspan : a.W);
+        p.span_stride = a.Wspan ? a.span_stride : Q::TS;
+    } else {
+        p.row_bytes = a.K / Q::BS * Q::TS;
+        p.Wspan = reinterpret_cast<const uint8_t *>(a.Wspan);
+        p.span_stride = a.span_stride;
+    }
     p.loraU = a.lora.T ? reinterpret_cast<const uint16_t *>(a.lora.U) : nullptr;
     p.ldu = a.lora.ldu;
     p.lora_kb = a.lora.kblocks;
@@ -286,7 +296,10 @@ static int tmem_launch(const TmemArgs &a, const TmemPlan &pl, float *partial)
     p.ftiles = 2 * pl.ftiles;                        // 128-feature halves of the 256-feature item
     p.ttiles = pl.ttiles * pl.accs;                  // TT-token parts of the TT * ACCS-token item
     p.kb_per_split = 4 * pl.spans_per_split;
-    p.kb_total = 4 * (int)((a.K + kSpan - 1) / kSpan);
+    p.kb_total = a.straddled ? (int)(a.K / kBlockK) : 4 * (int)((a.K + kSpan - 1) / kSpan);
+    if constexpr (Q::BS == 256) {
+        if (a.straddled) return wg_launch<Q, Prod, ACT, TT, true, true>(tmX, tmX, tmT, p, pl.splits, a.st);
+    }
     return wg_launch<Q, Prod, ACT, TT, true>(tmX, tmX, tmT, p, pl.splits, a.st);
 }
 
@@ -324,17 +337,20 @@ template <class Q, int ACT> static int tmem_run(const TmemArgs &a)
 
 // The hand-written producers read the canonical packed rows with 16-byte loads when one row's span and the row stride are
 // multiples of 16 B, and K is a whole number of k-blocks (a quarter of a span never reaches past the row); every other
-// weight needs the re-packed span-major layout of repack.cu
-template <class Q> static bool canonical_ok(const void *W, long long K)
+// weight needs the re-packed span-major layout of repack.cu.  A straddled weight has no rows to speak of: its blocks
+// (Q4_K 144 B, Q5_K 176 B) must be multiples of 16 B, and K a whole number of k-blocks, so that every k-block of every
+// row is one quarter of one block; the others need the block-major copy of repack.cu.
+template <class Q> static bool canonical_ok(const void *W, long long N, long long K)
 {
-    const long long row_bytes = K / Q::BS * Q::TS;
-    return SpanOf<Q>::BYTES % 16 == 0 && row_bytes % 16 == 0 && K % kBlockK == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0;
+    const bool aligned = SpanOf<Q>::BYTES % 16 == 0 && K % kBlockK == 0 && (reinterpret_cast<uintptr_t>(W) & 15) == 0;
+    if (straddled_rows(Q::BS, N, K)) return aligned;
+    return aligned && (K / Q::BS * Q::TS) % 16 == 0;
 }
 
 bool fused_tmem_supported(int type, const void *W, long long N, long long K)
 {
     if (N % 8 != 0 || K % 8 != 0) return false;
-    return with_block(type, false, [&](auto blk) { return canonical_ok<decltype(blk)>(W, K); });
+    return with_block(type, false, [&](auto blk) { return canonical_ok<decltype(blk)>(W, N, K); });
 }
 
 int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
@@ -342,10 +358,12 @@ int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span
                       const LinearOptions &opt, const LoraOperands &lora, cudaStream_t st)
 {
     if (N % 8 != 0 || K % 8 != 0) return GGUFB200_E_UNSUPPORTED;
-    const TmemArgs a{W, Wspan, span_stride, N, K, X, M, ldx, bias, bias_dtype, Y, ldy, ws, ws_bytes, opt, lora, st};
     return with_block(type, GGUFB200_E_UNSUPPORTED, [&](auto blk) {
         using Q = decltype(blk);
-        if (!Wspan && !canonical_ok<Q>(W, K)) return GGUFB200_E_UNSUPPORTED;
+        const bool straddled = straddled_rows(Q::BS, N, K);
+        if (straddled && K % kBlockK != 0) return GGUFB200_E_UNSUPPORTED;       // a k-block would span two blocks
+        if (!Wspan && !canonical_ok<Q>(W, N, K)) return GGUFB200_E_UNSUPPORTED;
+        const TmemArgs a{W, Wspan, span_stride, N, K, X, M, ldx, bias, bias_dtype, Y, ldy, ws, ws_bytes, opt, lora, st, straddled};
         return act_dtype == kBF16 ? tmem_run<Q, kBF16>(a) : tmem_run<Q, kF16>(a);
     });
 }

@@ -6,7 +6,11 @@
 // One CTA computes one output tile for one K range.  Both operands are K-major 64-wide k-blocks in shared memory in the
 // 128-byte swizzle layout: the activation tile is loaded by the TMA engine (zero-filled past M and K), the weight tile either
 // by the TMA engine (Q = Prod = void) or by a producer warpgroup that runs Prod::run64 (produce.cuh) on the packed row bytes and
-// stores the result in the swizzled layout.  Orientation:
+// stores the result in the swizzled layout.  STRADDLED (TRANS, 256-element blocks only): the weight is a flat stream of blocks
+// whose rows start inside blocks (straddled_rows, internal.h); k-block kb of row n is quarter (e >> 6) & 3 of block e >> 8,
+// e = n K + 64 kb (K % 64 == 0), at Wspan + (e >> 8) * span_stride.  A template parameter, so that the row-addressed
+// instances are compiled exactly as without it.
+// Orientation:
 //   TRANS = false   A = 128 activation rows, B = TN weight rows       (D = token x feature)
 //   TRANS = true    A = 128 weight rows, B = TN activation rows       (D = feature x token; token tiles of 32 .. 256)
 // Warpgroup 0 produces, warpgroups 1 and 2 each own 64 rows of A and issue wgmma.m64nTNk16, keeping one k-block in flight.
@@ -32,8 +36,8 @@ struct WgParams {
     float *partial;          // split-K: fp32 [splits, M, N] (nullptr: final output)
     const uint8_t *W;        // canonical packed rows (Prod != void)
     long long row_bytes;
-    const uint8_t *Wspan;    // span-major copy (repack.cu) or nullptr
-    long long span_stride;   // bytes between consecutive spans of the span-major copy
+    const uint8_t *Wspan;    // span-major copy (repack.cu) or nullptr; STRADDLED: the block stream the producers read
+    long long span_stride;   // bytes between consecutive spans of the span-major copy; STRADDLED: bytes per block
     const uint16_t *loraU;   // fp16 [N, ldu] = scale * up: lora_kb extra k-blocks on the K range 0 (TRANS only)
     int ttiles, ftiles;      // output tiles along tokens / features; CTA = (split, ftile, ttile), token tile fastest
     int kb_per_split, kb_total;
@@ -67,7 +71,7 @@ template <int ACT> __device__ __forceinline__ uint32_t wg_h2_to_act(uint32_t h)
     }
 }
 
-template <class Q, class Prod, int ACT, int TN, bool TRANS>
+template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false>
 __global__ void __launch_bounds__(kWgThreads, 1)
 wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmT,
                  const WgParams p)
@@ -158,6 +162,10 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                             }
                             emit(half, o);
                         }
+                    } else if constexpr (STRADDLED) {
+                        static_assert(TRANS && Q::BS == 256, "straddled rows: FUSED_TMEM, 256-element blocks");
+                        const long long e = n * p.K + (long long)kb * kBlockK;
+                        Prod::run64(p.Wspan + (e >> 8) * p.span_stride, (int)(e >> 6) & 3, emit);
                     } else {
                         const int span = kb >> 2;
                         const uint8_t *src = p.Wspan ? p.Wspan + (long long)span * p.span_stride + n * SpanOf<Q>::PITCH
@@ -246,11 +254,11 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
 }
 
 // Launch one CTA per (split, feature tile, token tile).  tmT: LoRA T tile map (or a copy of tmX).
-template <class Q, class Prod, int ACT, int TN, bool TRANS>
+template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false>
 static int wg_launch(const CUtensorMap &tmX, const CUtensorMap &tmW, const CUtensorMap &tmT, const WgParams &p, int splits, cudaStream_t st)
 {
     using Cfg = WgCfg<TN, TRANS>;
-    auto kern = wg_linear_kernel<Q, Prod, ACT, TN, TRANS>;
+    auto kern = wg_linear_kernel<Q, Prod, ACT, TN, TRANS, STRADDLED>;
     static unsigned char attr[64] = {};
     if (!ensure_dynamic_smem(kern, Cfg::SMEM, attr)) return GGUFB200_E_CUDA;
     const long long ctas = (long long)p.ftiles * p.ttiles * splits;

@@ -13,6 +13,13 @@
 // The 128 rows of one CTA for one span are then 128*PITCH contiguous, 16-byte aligned bytes.  Pad bytes, rows >= N and the
 // tail of a ragged last span are zero (a zero block dequantises to 0 in every format).  The canonical bytes stay where
 // they are: GGMLTensor / state_dict semantics are untouched, the shadow is a cache the host layer may drop at any time.
+//
+// A straddled weight (straddled_rows(), internal.h: 256-element blocks, K % 256 != 0) is a flat stream of N*K/256 blocks
+// with no row boundaries to keep, so its shadow is BLOCK-major:
+//
+//     out[b][PITCH]         b = block index < N*K/256, zero padded (no row or span padding)
+//
+// and the FUSED_TMEM producers read block b at b * PITCH.
 #include "internal.h"
 #include "produce.cuh"
 
@@ -40,13 +47,17 @@ __global__ void __launch_bounds__(256) repack_kernel(const uint8_t *__restrict__
 template <class Q> static int repack_run(const void *W, long long N, long long K, void *out, cudaStream_t st)
 {
     constexpr int SPAN = SpanOf<Q>::BYTES, PITCH = SpanOf<Q>::PITCH;
-    const long long n_pad = (N + 255) / 256 * 256;
-    const int spans = (int)((K + 255) / 256);
+    // a straddled weight is copied as N*K/256 one-block "rows" of one span each (SPAN = TS for 256-element blocks)
+    const bool straddled = straddled_rows(Q::BS, N, K);
+    const long long rows = straddled ? N * K / 256 : N;
+    const long long n_pad = straddled ? rows : (N + 255) / 256 * 256;
+    const int spans = straddled ? 1 : (int)((K + 255) / 256);
+    const long long row_bytes = straddled ? Q::TS : K / Q::BS * Q::TS;
     const long long total = (long long)spans * n_pad * (PITCH / 2);
     long long blocks = (total + 255) / 256;
     const long long cap = (long long)sm_count() * 16;
     if (blocks > cap) blocks = cap;
-    repack_kernel<SPAN, PITCH><<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const uint8_t *>(W), N, n_pad, K / Q::BS * Q::TS, spans,
+    repack_kernel<SPAN, PITCH><<<(unsigned)blocks, 256, 0, st>>>(reinterpret_cast<const uint8_t *>(W), rows, n_pad, row_bytes, spans,
                                                                    reinterpret_cast<uint8_t *>(out));
     return cudaGetLastError() == cudaSuccess ? GGUFB200_OK : GGUFB200_E_CUDA;
 }
@@ -54,10 +65,18 @@ template <class Q> static int repack_run(const void *W, long long N, long long K
 // bytes of the shadow buffer and its geometry; 0 for types without a block layout
 size_t repack_bytes(int type, long long N, long long K, int *pitch, long long *span_stride)
 {
-    const int pt = with_block(type, 0, [](auto blk) { return SpanOf<decltype(blk)>::PITCH; });
+    int bs = 0;
+    const int pt = with_block(type, 0, [&](auto blk) {
+        bs = decltype(blk)::BS;
+        return SpanOf<decltype(blk)>::PITCH;
+    });
     if (pt == 0) return 0;
-    const long long n_pad = (N + 255) / 256 * 256;
     if (pitch) *pitch = pt;
+    if (straddled_rows(bs, N, K)) {                 // block-major
+        if (span_stride) *span_stride = pt;
+        return (size_t)(N * K / 256) * (size_t)pt;
+    }
+    const long long n_pad = (N + 255) / 256 * 256;
     if (span_stride) *span_stride = n_pad * pt;
     return (size_t)((K + 255) / 256) * (size_t)n_pad * (size_t)pt;
 }

@@ -118,13 +118,23 @@ _F16_CODE = _lib.F16
 
 def needs_span_layout(qtype, K):
     """True when the canonical GGUF rows cannot be staged by a 2-D tensor map (a row's 256-wide K-span or the row stride is
-    not a multiple of 16 bytes): Q2_K / Q3_K / Q6_K / IQ4_XS always, the others for some K (Q8_0 at K = 2432)."""
+    not a multiple of 16 bytes): Q2_K / Q3_K / Q6_K / IQ4_XS always, the others for some K (Q8_0 at K = 2432).
+    The answer holds for a straddled weight too (SD1.5 / SDXL K-quants at K % 256 != 0, whose 256-element blocks straddle
+    rows): the kernel reads Q4_K / Q5_K from the canonical block stream and the other four from a block-major copy."""
     bs, ts = gguf.GGML_QUANT_SIZES[qtype]
     return bs > 1 and (((256 // bs) * ts) % 16 != 0 or ((K // bs) * ts) % 16 != 0)
 
 
+def straddled_rows(qtype, K):
+    """True for a weight whose 256-element blocks straddle rows (csrc/internal.h): K % 256 != 0 with a K-quant, the flat block
+    stream the GGUF converter writes for SD1.5 / SDXL tensors.  The library serves it by dequant + GEMM unless a route is asked
+    for (FUSED_TMEM, which the in-kernel LoRA takes)."""
+    return gguf.GGML_QUANT_SIZES[qtype][0] == 256 and K % 256 != 0
+
+
 def span_layout(weight, wraw):
-    """The re-packed span-major copy of a device-resident packed weight (csrc/repack.cu, SURVEY 8f rank 3), built once and
+    """The re-packed span-major copy of a device-resident packed weight (csrc/repack.cu, SURVEY 8f rank 3; block-major for a
+    straddled weight), built once and
     cached ON the GGMLTensor object: `.to()` / reload create new tensor objects, so the cache can never outlive its bytes.
     The canonical bytes are untouched (state_dict / offload semantics stay the reference's)."""
     key = (wraw.data_ptr(), wraw._version)
@@ -473,6 +483,7 @@ class GGMLOps(comfy_ops.manual_cast):
         # Weights whose canonical rows the TMA engine cannot stage (Q2_K / Q3_K / Q6_K / IQ4_XS, Q8_0 at K = 2432 ...) get a
         # re-packed span-major shadow copy on first use (one extra copy of the packed bytes in HBM, csrc/repack.cu) so that
         # they too run on the FUSED_TMEM kernel; False keeps them on the round-1 routes (smem-fed fused / dequant + dense GEMM).
+        # Straddled weights (`straddled_rows`) get no copy: dequant + dense GEMM was the faster route for them at every M measured.
         repack_spans = True
 
         def _fused_ok(self, input):
@@ -576,7 +587,7 @@ class GGMLOps(comfy_ops.manual_cast):
                     exact = (_lib.FLAG_EXACT_W if self.linear_numerics != "fast" else 0) | _lib.FLAG_W_STABLE
                     algo |= exact
                     if (self.repack_spans and resident and math == _F16_CODE and N % 8 == 0 and qtype != _Q.BF16
-                            and needs_span_layout(qtype, K) and M > GEMV_MAX_M):
+                            and needs_span_layout(qtype, K) and M > GEMV_MAX_M and not straddled_rows(qtype, K)):
                         spans = span_layout(w, wraw)                   # cached on the tensor after the first forward
                         algo = _lib.ALGO_FUSED_TMEM | exact
                     lora = None

@@ -39,7 +39,7 @@ extern "C" {
 #define GGUFB200_E_TYPE (-1)      /* ggml_type not in dequant.py:287-301 */
 #define GGUFB200_E_DTYPE (-2)     /* dtype code out of range */
 #define GGUFB200_E_ALIGN (-3)     /* output / activation pointer not 16-byte aligned */
-#define GGUFB200_E_SHAPE (-4)     /* K not a multiple of the block size, negative size, ld too small ... */
+#define GGUFB200_E_SHAPE (-4)     /* K not a multiple of the block size (nor a straddled weight), negative size, ld too small ... */
 #define GGUFB200_E_NULL (-5)      /* required pointer is NULL */
 #define GGUFB200_E_CUDA (-6)      /* a CUDA call failed (cudaGetLastError preserved for the caller) */
 #define GGUFB200_E_WORKSPACE (-7) /* workspace smaller than ggufb200_linear_workspace() */
@@ -147,7 +147,13 @@ int ggufb200_dequant_rows(int ggml_type, const void *packed, int64_t n_table_row
  * Fused Linear: Y[M,N] = X[M,K] * dequant(W)[N,K]^T (+ bias[N]).  Replaces
  * ops.py:242-244 `forward_ggml_cast_weights` = cast_bias_weight (ops.py:193-211)
  * -> get_weight/dequantize_tensor (ops.py:166-191) -> F.linear.
- *   W_packed    N rows of K/block_size*type_size bytes (loader.py:118-120 layout)
+ *   W_packed    N rows of K/block_size*type_size bytes (loader.py:118-120 layout), or a STRADDLED weight: 256-element
+ *               blocks, K % 256 != 0, N*K % 256 == 0, K % 8 == 0 -- the flat stream of N*K/256 blocks the GGUF converter
+ *               writes for SD1.5 / SDXL tensors (reshaped to [N*K/256, 256] before quantising), row n starting at element
+ *               n*K, possibly inside a block.  AUTO serves a straddled weight by GGUFB200_ALGO_DEQUANT_MMA (measured the
+ *               faster route, DESIGN.md section 9); GGUFB200_ALGO_FUSED_TMEM reads it when K % 64 == 0 (Q4_K / Q5_K from
+ *               the canonical bytes, the others with the block-major copy of ggufb200_repack()); GEMV, GEMV_FAST and
+ *               FUSED_MMA return GGUFB200_E_UNSUPPORTED.
  *   X, Y        act_dtype (0 fp16 / 1 bf16), row strides ldx / ldy in ELEMENTS, 16-byte aligned
  *   math_dtype  as in ggufb200_dequant().  Routes 1-3: W is first produced in math_dtype with the reference's rounding
  *               sequence and then cast to act_dtype, exactly the weight the reference hands to F.linear.  Route 4
@@ -181,6 +187,8 @@ int ggufb200_linear(int ggml_type, const void *W_packed, int64_t N, int64_t K, c
  * filled) that GGUFB200_ALGO_FUSED_TMEM reads with 16-byte loads for EVERY block format and every K.  The
  * canonical bytes are not modified (GGMLTensor / state_dict semantics are the reference's); the copy is a cache owned by
  * the caller: ggufb200_repack_bytes() bytes, 16-byte aligned, valid as long as the caller keeps it.
+ * A straddled weight (see ggufb200_linear) gets a BLOCK-major copy instead: out[block][pitch] for the N*K/256 blocks of the
+ * stream, zero padded, N*K/256*pitch bytes (pitch 112 / 112 / 240 / 144 for Q2_K / Q3_K / Q6_K / IQ4_XS).
  * ggufb200_linear_spans() = ggufb200_linear() with that copy at hand: AUTO then takes the FUSED_TMEM kernel for every format
  * (W_packed is still required: the reference-exact routes and EXACT_W read the canonical bytes).
  */
