@@ -27,6 +27,13 @@ class GGUFB200Error(RuntimeError):
     pass
 
 
+class KronPatch(ctypes.Structure):
+    """ggufb200_kron_patch (include/ggufb200.h): one LoKr patch of ggufb200_dequant_kron."""
+    _fields_ = [("A", ctypes.c_void_p), ("B", ctypes.c_void_p), ("a1", ctypes.c_int64), ("a2", ctypes.c_int64), ("b1", ctypes.c_int64),
+                ("b2", ctypes.c_int64), ("band_dim", ctypes.c_int32), ("scale", ctypes.c_float), ("band_start", ctypes.c_int64),
+                ("band_size", ctypes.c_int64)]
+
+
 def build(verbose: bool = False) -> str:
     """Compile the CUDA sources in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     out = subprocess.run(["bash", os.path.join(_HERE, "csrc", "build.sh")], capture_output=True, text=True)
@@ -55,6 +62,7 @@ def lib() -> ctypes.CDLL:
     L.ggufb200_supported.argtypes = [c_int, c_int]
     L.ggufb200_set_tuning.argtypes = [c_int, c_int]
     L.ggufb200_dequant.argtypes = [c_int, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
+    L.ggufb200_dequant_kron.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(KronPatch), c_int, c_vp]
     L.ggufb200_unpack_int.argtypes = [c_int, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]
     L.ggufb200_dequant_rows.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
     L.ggufb200_linear_plan.restype = c_int
@@ -90,5 +98,5 @@ EXPORTS = (
     "ggufb200_unpack_int", "ggufb200_dequant_rows", "ggufb200_linear_workspace", "ggufb200_linear", "ggufb200_gemm",
     "ggufb200_set_tuning", "ggufb200_linear_plan", "ggufb200_linear_workspace_ex",
     "ggufb200_repack_bytes", "ggufb200_repack", "ggufb200_linear_spans", "ggufb200_linear_lora",
-    "ggufb200_linear_lora_ex",
+    "ggufb200_linear_lora_ex", "ggufb200_dequant_kron",
 )

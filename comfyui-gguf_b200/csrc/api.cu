@@ -188,7 +188,40 @@ int ggufb200_dequant(int ggml_type, const void *packed, int64_t n_blocks, void *
     return dequant_dispatch(ggml_type, packed, n_blocks, out, out_dtype, math_dtype, (cudaStream_t)stream, stable);
 }
 
-int ggufb200_unpack_int(int ggml_type, const void *packed, int64_t n_blocks, int16_t *q, int16_t *sc, int16_t *mn, void *stream)
+int ggufb200_dequant_kron(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
+                          const ggufb200_kron_patch *patches, int n_patches, void *stream)
+{
+    int bs;
+    if (!type_geom(ggml_type, &bs, nullptr)) return GGUFB200_E_TYPE;
+    if (ggml_type == T_BF16) return GGUFB200_E_UNSUPPORTED;
+    const bool stable = (math_dtype & GGUFB200_DEQUANT_SRC_STABLE) != 0;
+    math_dtype &= ~GGUFB200_DEQUANT_SRC_STABLE;
+    if (!dtype_ok(out_dtype) || !dtype_ok(math_dtype)) return GGUFB200_E_DTYPE;
+    if (N <= 0 || K <= 0 || K % 8 != 0 || N > 0x7fffffffll || K > 0x7fffffffll || (K % bs != 0 && !straddled_rows(bs, N, K)))
+        return GGUFB200_E_SHAPE;
+    if (n_patches < 0 || n_patches > kKronMaxPatches) return GGUFB200_E_SHAPE;
+    if (n_patches > 0 && !patches) return GGUFB200_E_NULL;
+    for (int i = 0; i < n_patches; ++i) {
+        const ggufb200_kron_patch &p = patches[i];
+        const int64_t dim = p.band_dim;
+        if (dim < -1 || dim > 1 || p.a1 <= 0 || p.a2 <= 0 || p.b1 <= 0 || p.b2 <= 0) return GGUFB200_E_SHAPE;
+        int64_t rows = N, cols = K;
+        if (dim >= 0) {
+            const int64_t extent = dim == 0 ? N : K;
+            if (p.band_start < 0 || p.band_size <= 0 || p.band_start > extent - p.band_size) return GGUFB200_E_SHAPE;
+            (dim == 0 ? rows : cols) = p.band_size;
+        }
+        if (p.a1 > rows || p.b1 > rows || p.a2 > cols || p.b2 > cols || p.a1 * p.b1 != rows || p.a2 * p.b2 != cols) return GGUFB200_E_SHAPE;
+        if (!p.A || !p.B) return GGUFB200_E_NULL;
+        if ((reinterpret_cast<uintptr_t>(p.A) & 3) || (reinterpret_cast<uintptr_t>(p.B) & 3)) return GGUFB200_E_ALIGN;
+    }
+    if (!packed || !out) return GGUFB200_E_NULL;
+    if (!aligned16(out)) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    return dequant_kron_dispatch(ggml_type, packed, N, K, out, out_dtype, math_dtype, patches, n_patches, (cudaStream_t)stream, stable);
+}
+
+int ggufb200_unpack_int(int ggml_type,const void *packed, int64_t n_blocks, int16_t *q, int16_t *sc, int16_t *mn, void *stream)
 {
     if (!type_geom(ggml_type, nullptr, nullptr) || ggml_type == T_BF16) return GGUFB200_E_TYPE;
     if (n_blocks < 0) return GGUFB200_E_SHAPE;

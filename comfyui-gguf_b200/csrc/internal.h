@@ -6,6 +6,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "../../include/ggufb200.h"
+
 namespace ggufb200 {
 
 // ------------------------------------------------------------------ tuning switches (ggufb200_set_tuning)
@@ -17,6 +19,11 @@ int dequant_dispatch(int type, const void *packed, long long n_blocks, void *out
 int unpack_dispatch(int type, const void *packed, long long n_blocks, int16_t *q, int16_t *sc, int16_t *mn, cudaStream_t st);
 int rows_dispatch(int type, const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows, void *out,
                   int out_dtype, int math_dtype, cudaStream_t st);
+// ggufb200_dequant_kron: the [N, K] weight (whole-block rows or straddled, K % 8 == 0) with LoKr patches applied; `patches` are
+// validated by the caller (api.cu), n_patches <= kKronMaxPatches
+constexpr int kKronMaxPatches = 8;
+int dequant_kron_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
+                          const ggufb200_kron_patch *patches, int n_patches, cudaStream_t st, bool stable);
 
 // ------------------------------------------------------------------ small-M Linear: gemv.cu (GGUFB200_ALGO_GEMV), gemv2.cu (GEMV_FAST)
 int gemv_max_m();

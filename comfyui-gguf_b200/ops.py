@@ -155,6 +155,7 @@ def span_layout(weight, wraw):
 
 LORA_MAX_RANK = 64     # width of one LoRA k-block of the FUSED_TMEM kernel
 LORA_KERNEL_MAX_RANK = 8 * LORA_MAX_RANK     # at most 8 LoRA k-blocks: a larger total rank takes the side GEMMs (`_add_lora`)
+KRON_MAX_PATCHES = 8   # LoKr patches one ggufb200_dequant_kron call applies (csrc/internal.h kKronMaxPatches); more -> two-step route
 
 
 def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None):
@@ -316,6 +317,104 @@ def lora_band_terms(patches):
         scale = float(entry[0]) * (1.0 if alpha is None else float(alpha) / down.shape[0])
         terms.append((scale, up, down, band))
     return terms
+
+
+def lycoris_terms(patches):
+    """Recognise a patch list of LoRA, LoHa and LoKr (LyCORIS) entries, in any mix.
+
+    Entries follow comfy.lora's layout (see `lora_side_terms`); a LoHa value is `("loha", (w1a, w1b, alpha, w2a, w2b, t1, t2,
+    dora_scale))` or a LoHaAdapter carrying that tuple in `.weights`, a LoKr value `("lokr", (w1, w2, alpha, w1_a, w1_b, w2_a, w2_b,
+    t2, dora_scale))` or a LoKrAdapter.  Returns [(kind, scale, factors, band), ...] in list order:
+        "lora"  factors (up, down)                          scale as `lora_band_terms`
+        "loha"  factors (w1a, w1b, w2a, w2b)                scale = strength * alpha / w1b.shape[0] (strength when alpha is None)
+        "lokr"  factors (w1, w2, w1_a, w1_b, w2_a, w2_b),   w1 or (w1_a, w1_b) given, likewise w2;  scale = strength * alpha / dim
+                with dim = w1_b.shape[0] when w1 is decomposed, w2_b.shape[0] when w2 is (that one wins), strength when alpha is
+                None or neither is decomposed
+    which is how comfy.lora.calculate_weight scales them.  band as `lora_band_terms`.  None when any entry needs the general
+    machinery: strength_model != 1, a function hook, another offset, Tucker factors (t1 / t2), DoRA, factors that are not 2-D
+    or do not chain, any other patch kind."""
+    def mat(t):
+        return torch.is_tensor(t) and t.dim() == 2
+
+    terms = []
+    for entry in patches:
+        lora = lora_band_terms([entry])
+        if lora is not None:
+            scale, up, down, band = lora[0]
+            terms.append(("lora", scale, (up, down), band))
+            continue
+        if len(entry) < 3 or entry[2] != 1.0 or (len(entry) > 4 and entry[4] is not None):
+            return None
+        offset = entry[3] if len(entry) > 3 else None
+        band = None
+        if offset is not None:
+            if not isinstance(offset, (tuple, list)) or len(offset) != 3 or offset[0] not in (0, 1):
+                return None
+            band = (int(offset[0]), int(offset[1]), int(offset[2]))
+            if band[1] < 0 or band[2] <= 0:
+                return None
+        value = entry[1]
+        kind = {"LoHaAdapter": "loha", "LoKrAdapter": "lokr"}.get(type(value).__name__)
+        if kind is not None and hasattr(value, "weights"):
+            payload = value.weights
+        elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] in ("loha", "lokr"):
+            kind, payload = value
+        else:
+            return None
+        strength = float(entry[0])
+        if kind == "loha":
+            if len(payload) < 5 or any(extra is not None for extra in payload[5:8]):
+                return None
+            w1a, w1b, alpha, w2a, w2b = payload[:5]
+            if not all(mat(t) for t in (w1a, w1b, w2a, w2b)) or w1a.shape[1] != w1b.shape[0] or w2a.shape[1] != w2b.shape[0] \
+                    or w1a.shape[0] != w2a.shape[0] or w1b.shape[1] != w2b.shape[1]:
+                return None
+            terms.append(("loha", strength * (1.0 if alpha is None else float(alpha) / w1b.shape[0]), (w1a, w1b, w2a, w2b), band))
+            continue
+        if len(payload) < 7 or any(extra is not None for extra in payload[7:9]):
+            return None
+        w1, w2, alpha, w1_a, w1_b, w2_a, w2_b = payload[:7]
+        dim = None
+        for whole, a, b in ((w1, w1_a, w1_b), (w2, w2_a, w2_b)):
+            if whole is not None:
+                if not mat(whole):
+                    return None
+            elif mat(a) and mat(b) and a.shape[1] == b.shape[0]:
+                dim = b.shape[0]
+            else:
+                return None
+        scale = strength * (float(alpha) / dim if alpha is not None and dim is not None else 1.0)
+        terms.append(("lokr", scale, (w1, w2, w1_a, w1_b, w2_a, w2_b), band))
+    return terms
+
+
+def lokr_factor_shapes(factors):
+    """(a1, a2), (b1, b2) of a recognised LoKr term's A = w1 (or w1_a @ w1_b) and B = w2 (or w2_a @ w2_b)."""
+    w1, w2, w1_a, w1_b, w2_a, w2_b = factors
+    a = tuple(w1.shape) if w1 is not None else (w1_a.shape[0], w1_b.shape[1])
+    b = tuple(w2.shape) if w2 is not None else (w2_a.shape[0], w2_b.shape[1])
+    return a, b
+
+
+def loha_as_lora(w1a, w1b, w2a, w2b, device):
+    """LoHa's (w1a @ w1b) * (w2a @ w2b) as one LoRA of rank r1 r2, in fp32: up[:, i r2 + j] = w1a[:, i] * w2a[:, j] and
+    down[i r2 + j, :] = w1b[i, :] * w2b[j, :]."""
+    f = [t.to(device=device, dtype=torch.float32) for t in (w1a, w1b, w2a, w2b)]
+    up = (f[0][:, :, None] * f[2][:, None, :]).reshape(f[0].shape[0], -1)
+    down = (f[1][:, None, :] * f[3][None, :, :]).reshape(-1, f[1].shape[1])
+    return up, down
+
+
+def lokr_operands(factors, device):
+    """A, B of a LoKr term as comfy.lora.calculate_weight forms them: fp32 factors, a decomposed one as the fp32 torch.mm of its
+    halves on `device`."""
+    w1, w2, w1_a, w1_b, w2_a, w2_b = factors
+
+    def f32(t):
+        return t.to(device=device, dtype=torch.float32)
+    A = f32(w1) if w1 is not None else torch.mm(f32(w1_a), f32(w1_b))
+    B = f32(w2) if w2 is not None else torch.mm(f32(w2_a), f32(w2_b))
+    return A.contiguous(), B.contiguous()
 
 
 def lora_kernel_operands(terms, N, K, dtype, device):
@@ -537,6 +636,74 @@ class GGMLOps(comfy_ops.manual_cast):
             self.__dict__["_gg_lora"] = (key, operands)
             return operands
 
+        def _lycoris_terms(self, dev):
+            """For a patch list with LoHa / LoKr entries (`lycoris_terms`, any mix with LoRA): (LoRA terms, LoKr patches) with the
+            LoHa entries as LoRA terms of rank r1 r2 and each LoKr entry as (scale, A, B, band), fp32 A / B on `dev`; both built
+            once per patch set.  None -> two-step route (also for patch_dtype other than None: the reference then forms the
+            delta in another dtype)."""
+            w = self.weight
+            if not self.lora_side_gemm or self.patch_dtype is not None:
+                return None
+            entries = []
+            for patch_list, _key in w.patches:
+                entries.extend(patch_list)
+            terms = lycoris_terms(entries)
+            if terms is None:
+                return None
+            N, K = tuple(w.tensor_shape)
+            for kind, _s, factors, band in terms:
+                rows, cols = N, K
+                if band is not None:
+                    dim, start, size = band
+                    if start + size > (N, K)[dim]:
+                        return None
+                    rows, cols = (size, K) if dim == 0 else (N, size)
+                if kind == "lokr":
+                    (a1, a2), (b1, b2) = lokr_factor_shapes(factors)
+                    if a1 * b1 != rows or a2 * b2 != cols:
+                        return None
+                else:
+                    up, down = factors[0], factors[-1]      # LoRA (up, down); LoHa: w1a and w2b carry the shape
+                    if up.shape[0] != rows or down.shape[1] != cols:
+                        return None
+            # identity + storage + version of every factor, as for `_lora_operands`
+            key = tuple((kind, float(scale), band) + tuple((id(t), t.data_ptr(), t._version, tuple(t.shape)) if t is not None else None
+                                                            for t in factors) for kind, scale, factors, band in terms) + (str(dev),)
+            cached = self.__dict__.get("_gg_lycoris")
+            if cached is not None and cached[0] == key:
+                return cached[1]
+            lora, kron = [], []
+            for kind, scale, factors, band in terms:
+                if kind == "lora":
+                    lora.append((scale, factors[0], factors[1], band))
+                elif kind == "loha":
+                    lora.append((scale, *loha_as_lora(*factors, dev), band))
+                else:
+                    kron.append((scale, *lokr_operands(factors, dev), band))
+            descs = (_lib.KronPatch * max(1, len(kron)))(*[
+                _lib.KronPatch(A.data_ptr(), B.data_ptr(), A.shape[0], A.shape[1], B.shape[0], B.shape[1], -1 if band is None else band[0],
+                               scale, 0 if band is None else band[1], 0 if band is None else band[2])
+                for scale, A, B, band in kron])
+            operands = (lora, (kron, descs) if kron else None)
+            self.__dict__["_gg_lycoris"] = (key, operands)
+            return operands
+
+        def _kron_linear(self, input, wraw, qtype, N, K, bias, kron):
+            """ggufb200_dequant_kron (the patched weight, bit-identical to the reference's) into an [N, K] workspace, then
+            ggufb200_gemm with the bias."""
+            patches, descs = kron
+            dev = input.device
+            if not wraw.is_contiguous():
+                wraw = wraw.contiguous()
+            W = torch.empty(N, K, dtype=input.dtype, device=dev)
+            # the packed weight is a parameter (or its host-to-device copy): never written by a kernel in flight
+            math = math_code(self.dequant_dtype, input.dtype) | _lib.DEQUANT_SRC_STABLE
+            with torch.cuda.device(dev):
+                rc = _lib.lib().ggufb200_dequant_kron(int(qtype), wraw.data_ptr(), N, K, W.data_ptr(), dtype_code(input.dtype), math, descs,
+                                                      len(patches), _current_stream_ptr(dev.index))
+            _lib.check(rc, f"ggufb200_dequant_kron({getattr(qtype, 'name', qtype)}, N={N}, K={K})")
+            return linear_dense(input, W, bias)
+
         def _add_lora(self, y, input, terms):
             x2 = input.reshape(-1, input.shape[-1])
             y2 = y.view(-1, y.shape[-1])
@@ -559,7 +726,13 @@ class GGMLOps(comfy_ops.manual_cast):
             return y
 
         def forward_ggml_cast_weights(self, input):
-            terms = self._lora_terms(input.device) if self._fused_ok(input) else None
+            fused = self._fused_ok(input)
+            terms = self._lora_terms(input.device) if fused else None
+            kron = None
+            if terms is None and fused and getattr(self.weight, "patches", None):
+                lycoris = self._lycoris_terms(input.device)           # LoHa / LoKr entries: LoRA terms + LoKr patches
+                if lycoris is not None:
+                    terms, kron = lycoris
             if terms is not None:
                 dev = input.device
                 w = self.weight
@@ -577,6 +750,10 @@ class GGMLOps(comfy_ops.manual_cast):
                 y = None
                 if M < 0:
                     pass                                               # feature mismatch: let F.linear raise the usual error
+                elif kron is not None:
+                    # LoKr: the patched weight in one K1 launch + the dense GEMM at every M; LoRA / LoHa terms as side GEMMs
+                    if qtype != _Q.BF16 and N % 8 == 0 and K % 8 == 0 and len(kron[0]) <= KRON_MAX_PATCHES:
+                        y = self._kron_linear(input, wraw, qtype, N, K, b, kron)
                 elif qtype == _Q.BF16 and M > GEMV_MAX_M:
                     if input.dtype == torch.bfloat16 and K % 8 == 0 and N % 8 == 0:   # already dense: straight to the tensor-core GEMM
                         y = linear_dense(input, wraw.view(torch.bfloat16).view(N, K), b)

@@ -126,6 +126,32 @@ int ggufb200_dequant(int ggml_type, const void *packed, int64_t n_blocks, void *
                      int math_dtype, void *stream);
 
 /*
+ * Standalone dequant of an [N, K] weight with LoKr (LyCORIS Kronecker) patches applied.  Replaces, for a LoKr-patched weight,
+ * the reference's dequantise + comfy.lora.calculate_weight: every element of `out` is the reference's patched weight
+ *     W'[n, k] = out( out(W[n, k]) + out( fp32(scale) * fp32(A[i1, i2] * B[j1, j2]) ) )
+ * with (i1, j1) = divmod(n - row0, b1) and (i2, j2) = divmod(k - col0, b2) inside the patch's band, out() = rounding to out_dtype
+ * and the sum formed in fp32; elements outside a band are left as they are.  Patches are applied in list order, one rounding
+ * each, as `weight += ((strength * alpha) * kron(w1, w2)).to(dtype)` does per patch entry.  W is the ggufb200_dequant value
+ * in math_dtype cast to out_dtype (math_dtype may carry GGUFB200_DEQUANT_SRC_STABLE).
+ *   packed     the rows of W: whole blocks per row, or a straddled weight (see ggufb200_linear); K % 8 == 0; not BF16
+ *   out        N*K elements of out_dtype, 16-byte aligned
+ *   patches    host array of n_patches (0 .. 8) descriptors; A and B are DEVICE pointers to row-major fp32 matrices
+ * Band: band_dim -1 = the whole weight (row0 = col0 = 0), 0 = output rows band_start .. band_start + band_size, 1 = input
+ * features band_start .. band_start + band_size (ComfyUI's patch `offset`).  a1*b1 and a2*b2 must equal the band's rows and
+ * columns (GGUFB200_E_SHAPE).  A / B must be 4-byte aligned (GGUFB200_E_ALIGN).
+ */
+typedef struct ggufb200_kron_patch {
+    const float *A;        /* [a1, a2]: LoKr w1 (or w1_a @ w1_b) */
+    const float *B;        /* [b1, b2]: LoKr w2 (or w2_a @ w2_b) */
+    int64_t a1, a2, b1, b2;
+    int32_t band_dim;      /* -1, 0 or 1 */
+    float scale;           /* strength * alpha */
+    int64_t band_start, band_size;
+} ggufb200_kron_patch;
+int ggufb200_dequant_kron(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
+                          const ggufb200_kron_patch *patches, int n_patches, void *stream);
+
+/*
  * Integer unpack only (test/debug surface for the "bit-exact integer unpack" contract):
  * per element the integer quant value q as it enters the float multiply, the integer
  * sub-block scale sc (1 if the type has none) and min mn (0 if none).  Any of the three
