@@ -20,7 +20,7 @@ ALGO_MASK = 0xFF
 FLAG_EXACT_W, FLAG_GENERIC, FLAG_TILE384, FLAG_NOSPLIT, FLAG_UNSTAGED, FLAG_TILE192 = 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000
 FLAG_W_STABLE = 0x4000          # ggufb200_linear: no kernel still in flight writes the packed weight (prefetch under the previous kernel's tail)
 DEQUANT_SRC_STABLE = 0x100      # same promise for ggufb200_dequant, OR-ed into math_dtype
-OP_DEQUANT, OP_LINEAR, OP_ROWS, OP_LINEAR_MMA = 0, 1, 2, 3
+OP_DEQUANT, OP_LINEAR, OP_ROWS, OP_LINEAR_MMA, OP_DEQUANT_FALLBACK = 0, 1, 2, 3, 4
 
 
 class GGUFB200Error(RuntimeError):
@@ -62,6 +62,7 @@ def lib() -> ctypes.CDLL:
     L.ggufb200_supported.argtypes = [c_int, c_int]
     L.ggufb200_set_tuning.argtypes = [c_int, c_int]
     L.ggufb200_dequant.argtypes = [c_int, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
+    L.ggufb200_dequant_fallback.argtypes = [c_int, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
     L.ggufb200_dequant_kron.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(KronPatch), c_int, c_vp]
     L.ggufb200_unpack_int.argtypes = [c_int, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]
     L.ggufb200_dequant_rows.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
@@ -98,5 +99,5 @@ EXPORTS = (
     "ggufb200_unpack_int", "ggufb200_dequant_rows", "ggufb200_linear_workspace", "ggufb200_linear", "ggufb200_gemm",
     "ggufb200_set_tuning", "ggufb200_linear_plan", "ggufb200_linear_workspace_ex",
     "ggufb200_repack_bytes", "ggufb200_repack", "ggufb200_linear_spans", "ggufb200_linear_lora",
-    "ggufb200_linear_lora_ex", "ggufb200_dequant_kron",
+    "ggufb200_linear_lora_ex", "ggufb200_dequant_kron", "ggufb200_dequant_fallback",
 )

@@ -5,6 +5,7 @@
 #include <stdlib.h>
 
 #include "blocks.cuh"
+#include "fallback.cuh"
 #include "internal.h"
 
 using namespace ggufb200;
@@ -146,6 +147,7 @@ int ggufb200_type_info(int ggml_type, int *block_size, int *type_size)
 
 int ggufb200_supported(int ggml_type, int op)
 {
+    if (op == GGUFB200_OP_DEQUANT_FALLBACK) return with_fallback_block(ggml_type, 0, [](auto) { return 1; });
     if (!type_geom(ggml_type, nullptr, nullptr)) return 0;
     switch (op) {
     case GGUFB200_OP_DEQUANT: return 1;
@@ -186,6 +188,19 @@ int ggufb200_dequant(int ggml_type, const void *packed, int64_t n_blocks, void *
     if (!aligned16(out)) return GGUFB200_E_ALIGN;
     if (int rc = device_check()) return rc;
     return dequant_dispatch(ggml_type, packed, n_blocks, out, out_dtype, math_dtype, (cudaStream_t)stream, stable);
+}
+
+int ggufb200_dequant_fallback(int ggml_type, const void *packed, int64_t n_blocks, void *out, int out_dtype, int flags, void *stream)
+{
+    if (!with_fallback_block(ggml_type, false, [](auto) { return true; })) return GGUFB200_E_TYPE;
+    if (flags & ~GGUFB200_DEQUANT_SRC_STABLE) return GGUFB200_E_UNSUPPORTED;
+    if (!dtype_ok(out_dtype)) return GGUFB200_E_DTYPE;
+    if (n_blocks < 0) return GGUFB200_E_SHAPE;
+    if (n_blocks == 0) return GGUFB200_OK;
+    if (!packed || !out) return GGUFB200_E_NULL;
+    if (!aligned16(out)) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    return fallback_dispatch(ggml_type, packed, n_blocks, out, out_dtype, (cudaStream_t)stream, (flags & GGUFB200_DEQUANT_SRC_STABLE) != 0);
 }
 
 int ggufb200_dequant_kron(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,

@@ -7,7 +7,7 @@ FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler
 mkdir -p build
 pids=()
 for f in api dequant rows gemv gemv2 linear_sm90 repack; do
-  if [ ! -f build/$f.o ] || [ $f.cu -nt build/$f.o ] || [ internal.h -nt build/$f.o ] || [ common.cuh -nt build/$f.o ] || [ blocks.cuh -nt build/$f.o ] || [ wgmma.cuh -nt build/$f.o ] || [ linear_sm90.cuh -nt build/$f.o ] || [ produce.cuh -nt build/$f.o ] || [ ../../include/ggufb200.h -nt build/$f.o ]; then
+  if [ ! -f build/$f.o ] || [ $f.cu -nt build/$f.o ] || [ internal.h -nt build/$f.o ] || [ common.cuh -nt build/$f.o ] || [ blocks.cuh -nt build/$f.o ] || [ wgmma.cuh -nt build/$f.o ] || [ linear_sm90.cuh -nt build/$f.o ] || [ produce.cuh -nt build/$f.o ] || [ fallback.cuh -nt build/$f.o ] || [ fallback_tables.h -nt build/$f.o ] || [ ../../include/ggufb200.h -nt build/$f.o ]; then
     ( $NVCC $FLAGS -c $f.cu -o build/$f.o > build/$f.log 2>&1 || { cat build/$f.log | grep -v "^ptxas info" | head -50; exit 1; } ) &
     pids+=($!)
   fi

@@ -15,9 +15,12 @@
 //   * every thread unpacks one run of 32 consecutive elements from shared memory (blocks.cuh) into its row of the output
 //     tile in shared memory, which leaves through ONE swizzled tensor-map store (cp.async.bulk.tensor.2d, SASS UTMASTG): no
 //     thread computes a global address, every HBM write is a full line, and the unpack runs with immediate offsets
+// The types the reference dequantises through gguf-py's numpy fallback (fallback.cuh) run on the same kernel: only the
+// per-thread unpack differs (fp32 values, rounded once to the output dtype).
 #include <type_traits>
 
 #include "blocks.cuh"
+#include "fallback.cuh"
 #include "internal.h"
 #include "wgmma.cuh"
 
@@ -47,28 +50,50 @@ __device__ __forceinline__ void dequant_tile(const uint8_t *tile, uint8_t *otile
     constexpr int OB = OutT<OUT>::bytes;
     constexpr int EPC = 16 / OB;                           // elements per 16-byte chunk: 8 or 4
     constexpr int CH = 32 / EPC;                           // chunks per thread: 4 or 8
-    constexpr int GROUP = GroupOf<Q>::value;
     const int blk_in_tile = (tid * 32) / Q::BS;
     const int e0 = (tid * 32) % Q::BS;
-    if (tid * 32 < tile_elems) {
-        const uint8_t *blk = tile + blk_in_tile * Q::TS;
-        const GroupScale<MATH> g0 = group_scale<Q, MATH>(blk, e0);
-        GroupScale<MATH> g1 = g0;
-        if constexpr (GROUP == 16) g1 = group_scale<Q, MATH>(blk, e0 + 16);
-        const uint32_t obase = smem_u32(otile) + tid * (32 * OB);
-        const uint32_t sw = (obase >> 7) & (CH - 1);       // the engine's swizzle key: shared-memory address bits 7-8 (64B mode) / 7-9 (128B mode)
+    if constexpr (IsFallback<Q>::value) {
+        // fallback.cuh: gguf-py's fp32 values, rounded once to the output dtype (the reference's `.to(dtype)`)
+        static_assert(MATH == kF32, "the fallback formats are decoded in fp32 only");
+        if (tid * 32 < tile_elems) {
+            float v[32];
+            Q::run32(tile + blk_in_tile * Q::TS, e0, v);
+            const uint32_t obase = smem_u32(otile) + tid * (32 * OB);
+            const uint32_t sw = (obase >> 7) & (CH - 1);
 #pragma unroll
-        for (int c = 0; c < CH; ++c) {
-            const int e = e0 + c * EPC;
-            const bool second = (GROUP == 16) && (c * EPC >= 16);
-            typename Math<MATH>::T2 v[EPC / 2];
-            dequant_elems<Q, MATH, EPC>(blk, e, second ? g1 : g0, v);
-            const uint32_t oaddr = obase + ((uint32_t)c ^ sw) * 16;
-            if constexpr (OUT == kF32) {
-                float2 f0 = Math<MATH>::to_f32x2(v[0]), f1 = Math<MATH>::to_f32x2(v[1]);
-                st_otile_v4(oaddr, __float_as_uint(f0.x), __float_as_uint(f0.y), __float_as_uint(f1.x), __float_as_uint(f1.y));
-            } else {
-                st_otile_v4(oaddr, pack16<OUT, MATH>(v[0]), pack16<OUT, MATH>(v[1]), pack16<OUT, MATH>(v[2]), pack16<OUT, MATH>(v[3]));
+            for (int c = 0; c < CH; ++c) {
+                const float *f = v + c * EPC;
+                const uint32_t oaddr = obase + ((uint32_t)c ^ sw) * 16;
+                if constexpr (OUT == kF32) {
+                    st_otile_v4(oaddr, __float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3]));
+                } else {
+                    st_otile_v4(oaddr, pack16<OUT, kF32>(make_float2(f[0], f[1])), pack16<OUT, kF32>(make_float2(f[2], f[3])),
+                                pack16<OUT, kF32>(make_float2(f[4], f[5])), pack16<OUT, kF32>(make_float2(f[6], f[7])));
+                }
+            }
+        }
+    } else {
+        constexpr int GROUP = GroupOf<Q>::value;
+        if (tid * 32 < tile_elems) {
+            const uint8_t *blk = tile + blk_in_tile * Q::TS;
+            const GroupScale<MATH> g0 = group_scale<Q, MATH>(blk, e0);
+            GroupScale<MATH> g1 = g0;
+            if constexpr (GROUP == 16) g1 = group_scale<Q, MATH>(blk, e0 + 16);
+            const uint32_t obase = smem_u32(otile) + tid * (32 * OB);
+            const uint32_t sw = (obase >> 7) & (CH - 1);       // the engine's swizzle key: shared-memory address bits 7-8 (64B mode) / 7-9 (128B mode)
+#pragma unroll
+            for (int c = 0; c < CH; ++c) {
+                const int e = e0 + c * EPC;
+                const bool second = (GROUP == 16) && (c * EPC >= 16);
+                typename Math<MATH>::T2 v[EPC / 2];
+                dequant_elems<Q, MATH, EPC>(blk, e, second ? g1 : g0, v);
+                const uint32_t oaddr = obase + ((uint32_t)c ^ sw) * 16;
+                if constexpr (OUT == kF32) {
+                    float2 f0 = Math<MATH>::to_f32x2(v[0]), f1 = Math<MATH>::to_f32x2(v[1]);
+                    st_otile_v4(oaddr, __float_as_uint(f0.x), __float_as_uint(f0.y), __float_as_uint(f1.x), __float_as_uint(f1.y));
+                } else {
+                    st_otile_v4(oaddr, pack16<OUT, MATH>(v[0]), pack16<OUT, MATH>(v[1]), pack16<OUT, MATH>(v[2]), pack16<OUT, MATH>(v[3]));
+                }
             }
         }
     }
@@ -495,6 +520,21 @@ int dequant_dispatch(int type, const void *packed, long long n_blocks, void *out
     }
     return with_block(type, GGUFB200_E_TYPE, [&](auto blk) {
         return dispatch_math<decltype(blk)>(packed, n_blocks, out, out_dtype, math_dtype, stable, st);
+    });
+}
+
+// ggufb200_dequant_fallback: the same kernel, fp32 math (fallback.cuh)
+int fallback_dispatch(int type, const void *packed, long long n_blocks, void *out, int out_dtype, cudaStream_t st, bool stable)
+{
+    if (n_blocks == 0) return GGUFB200_OK;
+    return with_fallback_block(type, (int)GGUFB200_E_TYPE, [&](auto blk) {
+        using Q = decltype(blk);
+        switch (out_dtype) {
+        case kF16: return launch_dequant<Q, kF32, kF16>(packed, n_blocks, out, stable, st);
+        case kBF16: return launch_dequant<Q, kF32, kBF16>(packed, n_blocks, out, stable, st);
+        case kF32: return launch_dequant<Q, kF32, kF32>(packed, n_blocks, out, stable, st);
+        }
+        return (int)GGUFB200_E_DTYPE;
     });
 }
 

@@ -16,6 +16,8 @@ extern int g_gemv2_ctas;       // gemv2.cu: CTAs per SM of the integer-pattern G
 
 // ------------------------------------------------------------------ dequant.cu, rows.cu
 int dequant_dispatch(int type, const void *packed, long long n_blocks, void *out, int out_dtype, int math_dtype, cudaStream_t st, bool stable = false);
+// ggufb200_dequant_fallback: K1 for the formats of fallback.cuh (fp32 math); arguments validated by the caller
+int fallback_dispatch(int type, const void *packed, long long n_blocks, void *out, int out_dtype, cudaStream_t st, bool stable);
 int unpack_dispatch(int type, const void *packed, long long n_blocks, int16_t *q, int16_t *sc, int16_t *mn, cudaStream_t st);
 int rows_dispatch(int type, const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows, void *out,
                   int out_dtype, int math_dtype, cudaStream_t st);

@@ -8,8 +8,12 @@ Reference surface mirrored (file:line in /root/reference):
 
 Every dequantisation is ONE launch of csrc/dequant.cu through the C ABI.  The result is
 bit-identical to the reference for each (math dtype, output dtype) pair because the kernel
-reproduces the reference's per-op rounding (see csrc/common.cuh).  There is no numpy / CPU
-fallback (dequant.py:24-28 is intentionally not reproduced): unsupported types raise.
+reproduces the reference's per-op rounding (see csrc/common.cuh).
+
+The types the reference hands to gguf-py's numpy code (dequant.py:24-28: IQ2_XXS ... NVFP4, FALLBACK_QTYPES)
+are dequantised by the same kernel on the GPU (csrc/fallback.cuh, `dequantize_fallback`), bit-identical to
+`gguf.quants.dequantize` followed by the cast.  Nothing is computed on the CPU: without a CUDA device they
+raise NotImplementedError, as every other unsupported type does.
 """
 from __future__ import annotations
 
@@ -24,6 +28,8 @@ _DT_CODE = {torch.float16: _lib.F16, torch.bfloat16: _lib.BF16, torch.float32: _
 _Q = gguf.GGMLQuantizationType
 SUPPORTED_QTYPES = (_Q.BF16, _Q.Q8_0, _Q.Q5_1, _Q.Q5_0, _Q.Q4_1, _Q.Q4_0, _Q.Q6_K, _Q.Q5_K, _Q.Q4_K, _Q.Q3_K, _Q.Q2_K,
                     _Q.IQ4_NL, _Q.IQ4_XS)
+# the types of the reference's `else` branch (dequant.py:24-28) that gguf-py can dequantise: ggufb200_dequant_fallback
+FALLBACK_QTYPES = (_Q.IQ2_XXS, _Q.IQ2_XS, _Q.IQ2_S, _Q.IQ3_XXS, _Q.IQ3_S, _Q.IQ1_S, _Q.IQ1_M, _Q.TQ1_0, _Q.TQ2_0, _Q.MXFP4, _Q.NVFP4)
 
 
 def is_torch_compatible(tensor):
@@ -108,12 +114,48 @@ def dequantize(data, qtype, oshape, dtype=None, out_dtype=None, src_stable=None)
     return out
 
 
+def dequantize_fallback(data, qtype, oshape, dtype=None, src_stable=None):
+    """dequant.py:24-28 on the GPU: `torch.from_numpy(gguf.quants.dequantize(data, qtype)).to(dtype)` for a type of
+    FALLBACK_QTYPES, in one launch of ggufb200_dequant_fallback.  gguf-py's fp32 values rounded once to `dtype`
+    (None = float32, as the reference's `.to(dtype=None)`); the result has shape `oshape` and lives on data's device."""
+    qtype = gguf.GGMLQuantizationType(qtype)
+    if qtype not in FALLBACK_QTYPES:
+        raise NotImplementedError(f"ggufb200: {qtype.name} is not one of the numpy-fallback types")
+    if not torch.cuda.is_available():
+        raise NotImplementedError(f"ggufb200: {qtype.name} needs a CUDA device; the reference's numpy fallback "
+                                  "(dequant.py:24-28) is deliberately not provided")
+    block_size, type_size = gguf.GGML_QUANT_SIZES[qtype]
+    out_dtype = torch.float32 if dtype is None else dtype
+    flags = _lib.DEQUANT_SRC_STABLE if (SRC_STABLE if src_stable is None else src_stable) else 0
+    raw = _as_bytes(data)
+    src_device = raw.device
+    if raw.device.type != "cuda":
+        raw = raw.to("cuda", non_blocking=False)
+    n_bytes = raw.numel()
+    if n_bytes % type_size != 0:
+        raise ValueError(f"packed size {n_bytes} is not a multiple of the {qtype.name} block size {type_size}")
+    n_blocks = n_bytes // type_size
+    out = torch.empty(n_blocks * block_size, dtype=out_dtype, device=raw.device)
+    with torch.cuda.device(raw.device):
+        rc = _lib.lib().ggufb200_dequant_fallback(int(qtype), raw.data_ptr(), n_blocks, out.data_ptr(), dtype_code(out_dtype), flags,
+                                                  _stream_ptr(raw.device))
+    _lib.check(rc, f"ggufb200_dequant_fallback({qtype.name})")
+    out = out.reshape(oshape)
+    if src_device.type != "cuda":
+        out = out.to(src_device)
+    return out
+
+
 def dequantize_tensor(tensor, dtype=None, dequant_dtype=None):
-    """dequant.py:15-28 with the final `.to(dtype)` folded into the kernel."""
+    """dequant.py:15-28 with the final `.to(dtype)` folded into the kernel.  FALLBACK_QTYPES take the reference's `else`
+    branch (dequant_dtype ignored, dtype=None -> float32) on the GPU; the shape is `tensor_shape`, not the byte-derived
+    one the reference returns there."""
     qtype = getattr(tensor, "tensor_type", None)
     oshape = getattr(tensor, "tensor_shape", tensor.shape)
     if qtype in TORCH_COMPATIBLE_QTYPES:
         return tensor.to(dtype)
+    if qtype in FALLBACK_QTYPES:
+        return dequantize_fallback(tensor.data, qtype, oshape, dtype)
     if qtype not in dequantize_functions:
         raise NotImplementedError(
             f"ggufb200: qtype {getattr(qtype, 'name', repr(qtype))} is not supported; the reference's numpy fallback "

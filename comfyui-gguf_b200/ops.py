@@ -23,7 +23,7 @@ import torch
 
 from . import _lib
 from ._host import comfy_lora, comfy_mm, comfy_ops
-from .dequant import dequantize_rows, dequantize_tensor, dtype_code, is_quantized, math_code
+from .dequant import FALLBACK_QTYPES, dequantize_fallback, dequantize_rows, dequantize_tensor, dtype_code, is_quantized, math_code
 
 _Q = gguf.GGMLQuantizationType
 _FUSED_ACT = (torch.float16, torch.bfloat16)
@@ -729,7 +729,7 @@ class GGMLOps(comfy_ops.manual_cast):
             fused = self._fused_ok(input)
             terms = self._lora_terms(input.device) if fused else None
             kron = None
-            if terms is None and fused and getattr(self.weight, "patches", None):
+            if terms is None and fused and getattr(self.weight, "patches", None) and self.weight.tensor_type not in FALLBACK_QTYPES:
                 lycoris = self._lycoris_terms(input.device)           # LoHa / LoKr entries: LoRA terms + LoKr patches
                 if lycoris is not None:
                     terms, kron = lycoris
@@ -750,6 +750,12 @@ class GGMLOps(comfy_ops.manual_cast):
                 y = None
                 if M < 0:
                     pass                                               # feature mismatch: let F.linear raise the usual error
+                elif qtype in FALLBACK_QTYPES:
+                    # numpy-fallback types (csrc/fallback.cuh): no fused kernel reads them, so K1 into an [N, K] activation-dtype
+                    # weight (the reference's fp32 -> dtype rounding) + the dense GEMM at every M; other shapes: two-step route
+                    if N % 8 == 0 and K % 8 == 0:
+                        W = dequantize_fallback(wraw, qtype, (N, K), input.dtype)
+                        y = linear_dense(input, W, b)
                 elif kron is not None:
                     # LoKr: the patched weight in one K1 launch + the dense GEMM at every M; LoRA / LoHa terms as side GEMMs
                     if qtype != _Q.BF16 and N % 8 == 0 and K % 8 == 0 and len(kron[0]) <= KRON_MAX_PATCHES:
@@ -794,7 +800,7 @@ class GGMLOps(comfy_ops.manual_cast):
                 out_dtype = None
             w = self.weight
             plain_case = (self.max_norm is None and not getattr(w, "patches", None) and input.is_cuda
-                          and len(getattr(w, "tensor_shape", ())) == 2)
+                          and len(getattr(w, "tensor_shape", ())) == 2 and getattr(w, "tensor_type", None) not in FALLBACK_QTYPES)
             if plain_case:
                 w = w if w.device == input.device else w.to(input.device)
                 # the reference passes the module itself as `input` to cast_bias_weight (ops.py:256), so a missing

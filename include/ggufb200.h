@@ -56,6 +56,7 @@ extern "C" {
 #define GGUFB200_OP_LINEAR 1
 #define GGUFB200_OP_ROWS 2
 #define GGUFB200_OP_LINEAR_MMA 3 /* large-M tensor-core path (fused or dequant+GEMM) available for this type */
+#define GGUFB200_OP_DEQUANT_FALLBACK 4 /* ggufb200_dequant_fallback() serves this type */
 
 /* algorithm selector for ggufb200_linear(): one GGUFB200_ALGO_* value, optionally OR-ed with GGUFB200_FLAG_* bits */
 #define GGUFB200_ALGO_AUTO 0
@@ -102,8 +103,9 @@ const char *ggufb200_strerror(int rc);
 /* Block geometry: replaces gguf.GGML_QUANT_SIZES[qtype] as used at dequant.py:34. */
 int ggufb200_type_info(int ggml_type, int *block_size, int *type_size);
 
-/* 1 if (ggml_type, op) is implemented, else 0.  Mirrors `qtype in dequantize_functions`
- * (dequant.py:21, 287-301).  There is no CPU/numpy fallback (dequant.py:24-28 is NOT reproduced). */
+/* 1 if (ggml_type, op) is implemented, else 0.  For ops 0-3 mirrors `qtype in dequantize_functions`
+ * (dequant.py:21, 287-301).  The types of the reference's numpy fallback (dequant.py:24-28) are served on the GPU by
+ * ggufb200_dequant_fallback() instead (op GGUFB200_OP_DEQUANT_FALLBACK); nothing is computed on the CPU. */
 int ggufb200_supported(int ggml_type, int op);
 
 /*
@@ -124,6 +126,22 @@ int ggufb200_supported(int ggml_type, int op);
 #define GGUFB200_DEQUANT_SRC_STABLE 0x100
 int ggufb200_dequant(int ggml_type, const void *packed, int64_t n_blocks, void *out, int out_dtype,
                      int math_dtype, void *stream);
+
+/*
+ * Standalone dequant of the types the reference serves only through gguf-py's numpy fallback (dequant.py:24-28,
+ * `torch.from_numpy(gguf.quants.dequantize(bytes, qtype)).to(dtype)`): IQ2_XXS=16 IQ2_XS=17 IQ3_XXS=18 IQ1_S=19 IQ3_S=21
+ * IQ2_S=22 IQ1_M=29 TQ1_0=34 TQ2_0=35 MXFP4=39 NVFP4=40.  Every element is gguf-py's `dequantize_blocks` value, computed in
+ * fp32 with its operation order, then rounded once (to nearest even) to out_dtype: bit-identical to the reference (NaN
+ * payloads aside).  There is no math dtype: the reference ignores dequant_dtype on this branch.
+ *   packed     n_blocks * type_size bytes, any alignment
+ *   out        n_blocks * block_size elements of out_dtype, 16-byte aligned
+ *   flags      0 or GGUFB200_DEQUANT_SRC_STABLE (as in ggufb200_dequant); any other bit: GGUFB200_E_UNSUPPORTED
+ * Any other ggml_type, including the types of ggufb200_dequant, returns GGUFB200_E_TYPE; ggufb200_supported(t,
+ * GGUFB200_OP_DEQUANT_FALLBACK) lists exactly these eleven.  ggufb200_type_info, GGUFB200_OP_DEQUANT, the Linear entry points
+ * and ggufb200_dequant_rows keep the reference's table (dequant.py:287-301) only.
+ */
+int ggufb200_dequant_fallback(int ggml_type, const void *packed, int64_t n_blocks, void *out, int out_dtype, int flags,
+                              void *stream);
 
 /*
  * Standalone dequant of an [N, K] weight with LoKr (LyCORIS Kronecker) patches applied.  Replaces, for a LoKr-patched weight,
