@@ -85,6 +85,10 @@ def lib() -> ctypes.CDLL:
     L.ggufb200_linear_lora_ex.argtypes = [c_int, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_i64, c_vp, c_i64, c_int,
                                           c_vp, c_vp, c_i64, c_vp, c_sz, c_int, c_vp]
     L.ggufb200_gemm.argtypes = [c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_i64, c_vp]
+    L.ggufb200_linear_lora_scaled.argtypes = [c_int, c_vp, c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_i64, c_vp, c_i64,
+                                              c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_sz, c_int, c_vp]
+    L.ggufb200_gemm_scaled.argtypes = [c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_vp, c_i64, c_vp]
+    L.ggufb200_scale_columns.argtypes = [c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]
     _lib = L
     return L
 
@@ -99,5 +103,6 @@ EXPORTS = (
     "ggufb200_unpack_int", "ggufb200_dequant_rows", "ggufb200_linear_workspace", "ggufb200_linear", "ggufb200_gemm",
     "ggufb200_set_tuning", "ggufb200_linear_plan", "ggufb200_linear_workspace_ex",
     "ggufb200_repack_bytes", "ggufb200_repack", "ggufb200_linear_spans", "ggufb200_linear_lora",
-    "ggufb200_linear_lora_ex", "ggufb200_dequant_kron", "ggufb200_dequant_fallback",
+    "ggufb200_linear_lora_ex", "ggufb200_dequant_kron", "ggufb200_dequant_fallback", "ggufb200_linear_lora_scaled",
+    "ggufb200_gemm_scaled", "ggufb200_scale_columns",
 )

@@ -1,6 +1,6 @@
 // api.cu -- the extern "C" boundary declared in include/ggufb200.h.
 // Argument validation and route selection live here; kernels live in dequant.cu / rows.cu / gemv.cu / gemv2.cu /
-// linear_sm90.cu / repack.cu (declared in internal.h).  Routing is a pure function of the call's arguments (algo | flags):
+// linear_sm90.cu / repack.cu / scale.cu (declared in internal.h).  Routing is a pure function of the call's arguments (algo | flags):
 // no process-wide routing state.
 #include <stdlib.h>
 
@@ -275,7 +275,7 @@ size_t ggufb200_linear_workspace(int ggml_type, int64_t M, int64_t N, int64_t K,
 
 static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans, int64_t N, int64_t K, const void *X, int64_t M, int64_t ldx,
                        int act_dtype, int math_dtype, const void *bias, int bias_dtype, void *Y, int64_t ldy, void *workspace,
-                       size_t workspace_bytes, int algo, void *stream, const LoraOperands *lora = nullptr)
+                       size_t workspace_bytes, int algo, void *stream, const LoraOperands *lora = nullptr, const float *scale = nullptr)
 {
     int bs, ts;
     if (!type_geom(ggml_type, &bs, &ts)) return GGUFB200_E_TYPE;
@@ -317,6 +317,7 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
             (reinterpret_cast<uintptr_t>(lora->tiles) & 3))
             return GGUFB200_E_ALIGN;
     }
+    if (scale && !aligned16(scale)) return GGUFB200_E_ALIGN;     // only the LoRA entry point passes one: FUSED_TMEM
     if (int rc = device_check()) return rc;
     cudaStream_t st = (cudaStream_t)stream;
 
@@ -334,7 +335,7 @@ static int linear_impl(int ggml_type, const void *W_packed, const void *W_spans,
         long long span_stride = 0;
         if (W_spans) repack_bytes(ggml_type, N, K, nullptr, &span_stride);
         return fused_tmem_linear(ggml_type, W_packed, W_spans, span_stride, N, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, workspace,
-                                 ws_avail, opt, lora ? *lora : LoraOperands{}, st);
+                                 ws_avail, opt, lora ? *lora : LoraOperands{}, st, scale);
     }
     case GGUFB200_ALGO_DEQUANT_MMA: {
         if (ws_avail < dense) return GGUFB200_E_WORKSPACE;
@@ -375,9 +376,18 @@ int ggufb200_linear_lora_ex(int ggml_type, const void *W_packed, const void *W_s
                             int lora_kblocks, const int32_t *tile_kblocks, void *Y, int64_t ldy, void *workspace, size_t workspace_bytes, int algo,
                             void *stream)
 {
+    return ggufb200_linear_lora_scaled(ggml_type, W_packed, W_spans, N, K, X, M, ldx, act_dtype, bias, bias_dtype, T, ldt, U, ldu, lora_kblocks,
+                                       tile_kblocks, nullptr, Y, ldy, workspace, workspace_bytes, algo, stream);
+}
+
+int ggufb200_linear_lora_scaled(int ggml_type, const void *W_packed, const void *W_spans, int64_t N, int64_t K, const void *X, int64_t M,
+                                int64_t ldx, int act_dtype, const void *bias, int bias_dtype, const void *T, int64_t ldt, const void *U,
+                                int64_t ldu, int lora_kblocks, const int32_t *tile_kblocks, const float *feature_scale, void *Y, int64_t ldy,
+                                void *workspace, size_t workspace_bytes, int algo, void *stream)
+{
     const LoraOperands lora{T, ldt, U, ldu, lora_kblocks, tile_kblocks};
     return linear_impl(ggml_type, W_packed, W_spans, N, K, X, M, ldx, act_dtype, kF16, bias, bias_dtype, Y, ldy, workspace, workspace_bytes, algo,
-                       stream, &lora);
+                       stream, &lora, feature_scale);
 }
 
 size_t ggufb200_repack_bytes(int ggml_type, int64_t N, int64_t K)
@@ -421,14 +431,33 @@ int ggufb200_linear_plan(int ggml_type, int64_t M, int64_t N, int64_t K, size_t 
 int ggufb200_gemm(const void *W, int64_t N, int64_t K, int64_t ldw, const void *X, int64_t M, int64_t ldx, int act_dtype,
                   const void *bias, int bias_dtype, void *Y, int64_t ldy, void *stream)
 {
+    return ggufb200_gemm_scaled(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, nullptr, Y, ldy, stream);
+}
+
+int ggufb200_gemm_scaled(const void *W, int64_t N, int64_t K, int64_t ldw, const void *X, int64_t M, int64_t ldx, int act_dtype,
+                         const void *bias, int bias_dtype, const float *feature_scale, void *Y, int64_t ldy, void *stream)
+{
     if (act_dtype != kF16 && act_dtype != kBF16) return GGUFB200_E_DTYPE;
     if (bias && !dtype_ok(bias_dtype)) return GGUFB200_E_DTYPE;
     if (M < 0 || N <= 0 || K <= 0 || K % 8 != 0 || ldw < K || ldx < K || ldy < N) return GGUFB200_E_SHAPE;
     if (M == 0) return GGUFB200_OK;
     if (!W || !X || !Y) return GGUFB200_E_NULL;
     if (!aligned16(W) || !aligned16(X) || !aligned16(Y) || (ldw % 8) || (ldx % 8) || (ldy % 8)) return GGUFB200_E_ALIGN;
+    if (feature_scale && !aligned16(feature_scale)) return GGUFB200_E_ALIGN;
     if (int rc = device_check()) return rc;
-    return dense_gemm(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, (cudaStream_t)stream);
+    return dense_gemm(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, (cudaStream_t)stream, feature_scale);
+}
+
+int ggufb200_scale_columns(const void *X, int64_t M, int64_t K, int64_t ldx, int act_dtype, const float *col_scale, void *Y, int64_t ldy,
+                           void *stream)
+{
+    if (act_dtype != kF16 && act_dtype != kBF16) return GGUFB200_E_DTYPE;
+    if (M < 0 || K <= 0 || K % 8 != 0 || ldx < K || ldy < K) return GGUFB200_E_SHAPE;
+    if (M == 0) return GGUFB200_OK;
+    if (!X || !col_scale || !Y) return GGUFB200_E_NULL;
+    if (!aligned16(X) || !aligned16(Y) || !aligned16(col_scale) || (ldx % 8) || (ldy % 8)) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    return scale_columns_dispatch(X, M, K, ldx, act_dtype, col_scale, Y, ldy, (cudaStream_t)stream);
 }
 
 }  // extern "C"

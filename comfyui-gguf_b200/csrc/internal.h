@@ -60,8 +60,9 @@ struct LinearOptions {
 
 // `ws_bytes` is the usable workspace at `ws`: 0 when the caller passed none or a misaligned one.
 // Dense GEMM: ggufb200_gemm and the GEMM half of GGUFB200_ALGO_DEQUANT_MMA.
+// scale: nullptr, or fp32 [N] (16-byte aligned) multiplied into each output feature before the bias (ggufb200_gemm_scaled).
 int dense_gemm(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx, int act_dtype,
-               const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st);
+               const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st, const float *scale = nullptr);
 // GGUFB200_ALGO_FUSED_MMA: reference-exact producers, the weight as the wide operand.
 size_t fused_mma_workspace(long long M, long long N, long long K, const LinearOptions &opt);
 void fused_mma_plan(long long M, long long N, long long K, size_t ws_bytes, const LinearOptions &opt, int *tile_rows, int *splits,
@@ -83,8 +84,13 @@ bool fused_tmem_supported(int type, const void *W, long long N, long long K);
 size_t fused_tmem_workspace(long long M, long long N, long long K, const LinearOptions &opt);
 void fused_tmem_plan(long long M, long long N, long long K, size_t ws_bytes, const LinearOptions &opt, int *tile_tokens, int *splits,
                      int *spans_per_split, int *items);
+// scale: as for dense_gemm (ggufb200_linear_lora_scaled)
 int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
                       long long ldx, int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes,
-                      const LinearOptions &opt, const LoraOperands &lora, cudaStream_t st);
+                      const LinearOptions &opt, const LoraOperands &lora, cudaStream_t st, const float *scale = nullptr);
+
+// ------------------------------------------------------------------ scale.cu: Y = act(fp32(X) * c[k]) (ggufb200_scale_columns)
+int scale_columns_dispatch(const void *X, long long M, long long K, long long ldx, int act_dtype, const float *col_scale, void *Y,
+                           long long ldy, cudaStream_t st);
 
 }  // namespace ggufb200

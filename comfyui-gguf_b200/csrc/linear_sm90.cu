@@ -29,6 +29,10 @@
 // Split-K (both fused routes): when the output tiles leave SMs idle, K is cut into ranges of whole 256-wide spans, one CTA
 // per (tile, range); each CTA stores its fp32 partial tile into its own slice of the caller's workspace ([S, M, N] fp32) and
 // wg_finalize_kernel adds the slices in ascending order.  Every packed byte is still read once per token tile.
+//
+// Feature scale (ggufb200_gemm_scaled, ggufb200_linear_lora_scaled): the dense GEMM and FUSED_TMEM can multiply each output
+// feature by an fp32 factor before the bias, Y = act(scale[n] * acc + bias[n]), in the epilogue or in the split-K finalize.
+// Only those two launchers instantiate the SCALED kernels; a NULL scale runs the unscaled instances.
 #include "internal.h"
 #include "linear_sm90.cuh"
 
@@ -53,9 +57,9 @@ static KRanges k_ranges(long long spans, long long s)
 static size_t partial_bytes(int splits, long long M, long long N) { return splits > 1 ? (size_t)splits * (size_t)M * (size_t)N * 4 : 0; }
 
 // ------------------------------------------------------------------ dense GEMM
-template <int ACT, int BN>
+template <int ACT, int BN, bool SCALED>
 static int dense_launch(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx, const void *bias,
-                        int bias_dtype, void *Y, long long ldy, cudaStream_t st)
+                        int bias_dtype, void *Y, long long ldy, cudaStream_t st, const float *scale)
 {
     CUtensorMap tmA, tmB;
     if (!make_kblock_map(&tmA, X, M, K, ldx, ACT, 128)) return GGUFB200_E_CUDA;
@@ -68,21 +72,30 @@ static int dense_launch(const void *W, long long N, long long K, long long ldw, 
     p.ftiles = (int)((N + BN - 1) / BN);
     p.kb_total = (int)((K + kBlockK - 1) / kBlockK);
     p.kb_per_split = p.kb_total;
-    return wg_launch<void, void, ACT, BN, false>(tmA, tmB, tmA, p, 1, st);
+    p.scale = scale;
+    return wg_launch<void, void, ACT, BN, false, false, SCALED>(tmA, tmB, tmA, p, 1, st);
 }
 
-int dense_gemm(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx, int act_dtype,
-               const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st)
+template <bool SCALED>
+static int dense_tiles(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx, int act_dtype,
+                       const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st, const float *scale)
 {
-    if (K % 8 != 0 || N % 8 != 0) return GGUFB200_E_UNSUPPORTED;
     // 256-wide feature tiles; 128 when that leaves most SMs idle (short activations such as a 512-token text stream)
     const long long tiles256 = ((M + 127) / 128) * ((N + 255) / 256);
     const bool narrow = tiles256 < sm_count();
     if (narrow)
-        return act_dtype == kBF16 ? dense_launch<kBF16, 128>(W, N, K, ldw, X, M, ldx, bias, bias_dtype, Y, ldy, st)
-                                  : dense_launch<kF16, 128>(W, N, K, ldw, X, M, ldx, bias, bias_dtype, Y, ldy, st);
-    return act_dtype == kBF16 ? dense_launch<kBF16, 256>(W, N, K, ldw, X, M, ldx, bias, bias_dtype, Y, ldy, st)
-                              : dense_launch<kF16, 256>(W, N, K, ldw, X, M, ldx, bias, bias_dtype, Y, ldy, st);
+        return act_dtype == kBF16 ? dense_launch<kBF16, 128, SCALED>(W, N, K, ldw, X, M, ldx, bias, bias_dtype, Y, ldy, st, scale)
+                                  : dense_launch<kF16, 128, SCALED>(W, N, K, ldw, X, M, ldx, bias, bias_dtype, Y, ldy, st, scale);
+    return act_dtype == kBF16 ? dense_launch<kBF16, 256, SCALED>(W, N, K, ldw, X, M, ldx, bias, bias_dtype, Y, ldy, st, scale)
+                              : dense_launch<kF16, 256, SCALED>(W, N, K, ldw, X, M, ldx, bias, bias_dtype, Y, ldy, st, scale);
+}
+
+int dense_gemm(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx, int act_dtype,
+               const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st, const float *scale)
+{
+    if (K % 8 != 0 || N % 8 != 0) return GGUFB200_E_UNSUPPORTED;
+    return scale ? dense_tiles<true>(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st, scale)
+                 : dense_tiles<false>(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st, nullptr);
 }
 
 // ------------------------------------------------------------------ GGUFB200_ALGO_FUSED_MMA
@@ -264,9 +277,10 @@ struct TmemArgs {
     const LoraOperands &lora;  // lora.T == nullptr: no LoRA k-blocks
     cudaStream_t st;
     bool straddled;            // straddled_rows(): W (or Wspan, the block-major copy) is a flat stream of 256-element blocks
+    const float *scale;        // fp32 [N] feature scale (SCALED instances) or nullptr
 };
 
-template <class Q, class Prod, int ACT, int TT>
+template <class Q, class Prod, int ACT, int TT, bool SCALED>
 static int tmem_launch(const TmemArgs &a, const TmemPlan &pl, float *partial)
 {
     CUtensorMap tmX, tmT;
@@ -293,21 +307,22 @@ static int tmem_launch(const TmemArgs &a, const TmemPlan &pl, float *partial)
     p.ldu = a.lora.ldu;
     p.lora_kb = a.lora.kblocks;
     p.lora_tiles = a.lora.tiles;
+    p.scale = partial ? nullptr : a.scale;           // split K: the finalize applies it
     p.ftiles = 2 * pl.ftiles;                        // 128-feature halves of the 256-feature item
     p.ttiles = pl.ttiles * pl.accs;                  // TT-token parts of the TT * ACCS-token item
     p.kb_per_split = 4 * pl.spans_per_split;
     p.kb_total = a.straddled ? (int)(a.K / kBlockK) : 4 * (int)((a.K + kSpan - 1) / kSpan);
     if constexpr (Q::BS == 256) {
-        if (a.straddled) return wg_launch<Q, Prod, ACT, TT, true, true>(tmX, tmX, tmT, p, pl.splits, a.st);
+        if (a.straddled) return wg_launch<Q, Prod, ACT, TT, true, true, SCALED>(tmX, tmX, tmT, p, pl.splits, a.st);
     }
-    return wg_launch<Q, Prod, ACT, TT, true>(tmX, tmX, tmT, p, pl.splits, a.st);
+    return wg_launch<Q, Prod, ACT, TT, true, false, SCALED>(tmX, tmX, tmT, p, pl.splits, a.st);
 }
 
-template <class Q, class Prod, int ACT> static int tmem_tiles(const TmemArgs &a, const TmemPlan &pl, float *partial)
+template <class Q, class Prod, int ACT, bool SCALED> static int tmem_tiles(const TmemArgs &a, const TmemPlan &pl, float *partial)
 {
-    if (pl.tt == 32) return tmem_launch<Q, Prod, ACT, 32>(a, pl, partial);
-    if (pl.tt == 128) return tmem_launch<Q, Prod, ACT, 128>(a, pl, partial);
-    return tmem_launch<Q, Prod, ACT, 192>(a, pl, partial);
+    if (pl.tt == 32) return tmem_launch<Q, Prod, ACT, 32, SCALED>(a, pl, partial);
+    if (pl.tt == 128) return tmem_launch<Q, Prod, ACT, 128, SCALED>(a, pl, partial);
+    return tmem_launch<Q, Prod, ACT, 192, SCALED>(a, pl, partial);
 }
 
 // does the fused-multiply-add flag change the hand-written producer of this format?  (only Q4_K / Q5_K have a two-rounding step)
@@ -315,24 +330,24 @@ template <class Q> struct FmaMatters {
     static constexpr bool value = Q::TS == 144 || Q::TS == 176;
 };
 
-template <class Q, int ACT> static int tmem_run(const TmemArgs &a)
+template <class Q, int ACT, bool SCALED> static int tmem_run(const TmemArgs &a)
 {
     const TmemPlan pl = tmem_plan(a.M, a.N, a.K, a.ws_bytes, a.opt.tile, !a.opt.nosplit);
     float *partial = pl.splits > 1 ? reinterpret_cast<float *>(a.ws) : nullptr;
     // the producer is chosen at compile time where the format leaves no choice, so no kernel is built that cannot be launched
     int rc;
     if constexpr (!FastProducer<Q>::fast) {
-        rc = tmem_tiles<Q, Producer<Q>, ACT>(a, pl, partial);                 // no hand-written producer for this format
+        rc = tmem_tiles<Q, Producer<Q>, ACT, SCALED>(a, pl, partial);                 // no hand-written producer for this format
     } else if (a.opt.producers == LinearOptions::GENERIC) {
-        rc = tmem_tiles<Q, Producer<Q>, ACT>(a, pl, partial);
+        rc = tmem_tiles<Q, Producer<Q>, ACT, SCALED>(a, pl, partial);
     } else if constexpr (FmaMatters<Q>::value) {
-        rc = a.opt.producers == LinearOptions::EXACT ? tmem_tiles<Q, FastProducer<Q, false>, ACT>(a, pl, partial)
-                                                     : tmem_tiles<Q, FastProducer<Q, true>, ACT>(a, pl, partial);
+        rc = a.opt.producers == LinearOptions::EXACT ? tmem_tiles<Q, FastProducer<Q, false>, ACT, SCALED>(a, pl, partial)
+                                                     : tmem_tiles<Q, FastProducer<Q, true>, ACT, SCALED>(a, pl, partial);
     } else {
-        rc = tmem_tiles<Q, FastProducer<Q, true>, ACT>(a, pl, partial);       // single-rounding step: FAST and EXACT coincide
+        rc = tmem_tiles<Q, FastProducer<Q, true>, ACT, SCALED>(a, pl, partial);       // single-rounding step: FAST and EXACT coincide
     }
     if (rc != GGUFB200_OK || !partial) return rc;
-    return wg_finalize<ACT>(partial, pl.splits, a.bias, a.bias_dtype, a.Y, a.M, a.N, a.ldy, a.st);
+    return wg_finalize<ACT, SCALED>(partial, pl.splits, a.bias, a.bias_dtype, a.Y, a.M, a.N, a.ldy, a.st, a.scale);
 }
 
 // The hand-written producers read the canonical packed rows with 16-byte loads when one row's span and the row stride are
@@ -355,7 +370,7 @@ bool fused_tmem_supported(int type, const void *W, long long N, long long K)
 
 int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
                       long long ldx, int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes,
-                      const LinearOptions &opt, const LoraOperands &lora, cudaStream_t st)
+                      const LinearOptions &opt, const LoraOperands &lora, cudaStream_t st, const float *scale)
 {
     if (N % 8 != 0 || K % 8 != 0) return GGUFB200_E_UNSUPPORTED;
     return with_block(type, GGUFB200_E_UNSUPPORTED, [&](auto blk) {
@@ -363,8 +378,9 @@ int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span
         const bool straddled = straddled_rows(Q::BS, N, K);
         if (straddled && K % kBlockK != 0) return GGUFB200_E_UNSUPPORTED;       // a k-block would span two blocks
         if (!Wspan && !canonical_ok<Q>(W, N, K)) return GGUFB200_E_UNSUPPORTED;
-        const TmemArgs a{W, Wspan, span_stride, N, K, X, M, ldx, bias, bias_dtype, Y, ldy, ws, ws_bytes, opt, lora, st, straddled};
-        return act_dtype == kBF16 ? tmem_run<Q, kBF16>(a) : tmem_run<Q, kF16>(a);
+        const TmemArgs a{W, Wspan, span_stride, N, K, X, M, ldx, bias, bias_dtype, Y, ldy, ws, ws_bytes, opt, lora, st, straddled, scale};
+        if (scale) return act_dtype == kBF16 ? tmem_run<Q, kBF16, true>(a) : tmem_run<Q, kF16, true>(a);
+        return act_dtype == kBF16 ? tmem_run<Q, kBF16, false>(a) : tmem_run<Q, kF16, false>(a);
     });
 }
 

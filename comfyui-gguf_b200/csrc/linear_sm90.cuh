@@ -16,7 +16,9 @@
 // Warpgroup 0 produces, warpgroups 1 and 2 each own 64 rows of A and issue wgmma.m64nTNk16, keeping one k-block in flight.
 // Ring: full[s] (TMA bytes + one arrive per producer warp), empty[s] (one arrive per consumer thread).
 // The epilogue either stores fp32 partial sums (split-K, summed by a finalize kernel in a fixed order) or adds the bias,
-// rounds to the activation dtype and writes the tile through shared memory with 16-byte stores.
+// rounds to the activation dtype and writes the tile through shared memory with 16-byte stores.  SCALED instances first
+// multiply each output feature by an fp32 factor: Y = act(scale[n] * acc + bias[n]) (DoRA's row norms, ggufb200_*_scaled);
+// a template parameter, so that the unscaled instances are compiled exactly as without it.
 #pragma once
 #include <type_traits>
 
@@ -44,6 +46,7 @@ struct WgParams {
     long long ldu;
     int lora_kb;             // LoRA k-blocks: T columns / U columns 64 j .. 64 j + 63, j < lora_kb
     const int *lora_tiles;   // per 128-feature tile (first, count): the LoRA k-blocks that tile runs; nullptr = all lora_kb
+    const float *scale;      // SCALED: fp32 [N] per-output-feature factor applied before the bias (final output only)
 };
 
 template <int TN, bool TRANS> struct WgCfg {
@@ -71,7 +74,7 @@ template <int ACT> __device__ __forceinline__ uint32_t wg_h2_to_act(uint32_t h)
     }
 }
 
-template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false>
+template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false, bool SCALED = false>
 __global__ void __launch_bounds__(kWgThreads, 1)
 wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmT,
                  const WgParams p)
@@ -234,6 +237,9 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                 const int ar = arow0 + 8 * h, bc = 8 * j + bcol0 + e;
                 const int tk = TRANS ? bc : ar, f = TRANS ? ar : bc;
                 float v = acc[4 * j + 2 * h + e];
+                if constexpr (SCALED) {
+                    if (feat0 + f < p.N) v *= p.scale[feat0 + f];
+                }
                 if (p.bias && feat0 + f < p.N) v += wg_bias<ACT>(p.bias, p.bias_dtype, feat0 + f);
                 uint16_t hb;
                 if constexpr (ACT == kBF16) hb = __bfloat16_as_ushort(__float2bfloat16_rn(v));
@@ -254,11 +260,11 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
 }
 
 // Launch one CTA per (split, feature tile, token tile).  tmT: LoRA T tile map (or a copy of tmX).
-template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false>
+template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false, bool SCALED = false>
 static int wg_launch(const CUtensorMap &tmX, const CUtensorMap &tmW, const CUtensorMap &tmT, const WgParams &p, int splits, cudaStream_t st)
 {
     using Cfg = WgCfg<TN, TRANS>;
-    auto kern = wg_linear_kernel<Q, Prod, ACT, TN, TRANS, STRADDLED>;
+    auto kern = wg_linear_kernel<Q, Prod, ACT, TN, TRANS, STRADDLED, SCALED>;
     static unsigned char attr[64] = {};
     if (!ensure_dynamic_smem(kern, Cfg::SMEM, attr)) return GGUFB200_E_CUDA;
     const long long ctas = (long long)p.ftiles * p.ttiles * splits;
@@ -267,10 +273,12 @@ static int wg_launch(const CUtensorMap &tmX, const CUtensorMap &tmW, const CUten
     return cudaGetLastError() == cudaSuccess ? GGUFB200_OK : GGUFB200_E_CUDA;
 }
 
-// split-K finalize: Y = act(sum_s P[s] + bias), slices added in ascending order (bit-reproducible)
-template <int ACT>
+// split-K finalize: Y = act(sum_s P[s] + bias), slices added in ascending order (bit-reproducible); SCALED:
+// Y = act(scale[n] * sum_s P[s] + bias)
+template <int ACT, bool SCALED = false>
 __global__ void __launch_bounds__(256) wg_finalize_kernel(const float *__restrict__ P, int splits, const void *__restrict__ bias, int bias_dtype,
-                                                          uint8_t *__restrict__ Y, long long M, long long N, long long ldy)
+                                                          uint8_t *__restrict__ Y, long long M, long long N, long long ldy,
+                                                          const float *__restrict__ scale)
 {
     const long long n8 = N / 8;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < M * n8; i += (long long)gridDim.x * 256) {
@@ -282,6 +290,11 @@ __global__ void __launch_bounds__(256) wg_finalize_kernel(const float *__restric
             v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w;
             v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
         }
+        if constexpr (SCALED) {
+            const float4 a = *reinterpret_cast<const float4 *>(scale + n), b = *reinterpret_cast<const float4 *>(scale + n + 4);
+            v[0] *= a.x; v[1] *= a.y; v[2] *= a.z; v[3] *= a.w;
+            v[4] *= b.x; v[5] *= b.y; v[6] *= b.z; v[7] *= b.w;
+        }
         if (bias) {
 #pragma unroll
             for (int j = 0; j < 8; ++j) v[j] += wg_bias<ACT>(bias, bias_dtype, n + j);
@@ -290,13 +303,14 @@ __global__ void __launch_bounds__(256) wg_finalize_kernel(const float *__restric
     }
 }
 
-template <int ACT>
-static int wg_finalize(const float *P, int splits, const void *bias, int bias_dtype, void *Y, long long M, long long N, long long ldy, cudaStream_t st)
+template <int ACT, bool SCALED = false>
+static int wg_finalize(const float *P, int splits, const void *bias, int bias_dtype, void *Y, long long M, long long N, long long ldy, cudaStream_t st,
+                       const float *scale = nullptr)
 {
     const long long work = M * (N / 8);
     const long long cap = (long long)sm_count() * 8;
     const unsigned grid = (unsigned)((work + 255) / 256 < cap ? (work + 255) / 256 : cap);
-    wg_finalize_kernel<ACT><<<grid, 256, 0, st>>>(P, splits, bias, bias_dtype, reinterpret_cast<uint8_t *>(Y), M, N, ldy);
+    wg_finalize_kernel<ACT, SCALED><<<grid, 256, 0, st>>>(P, splits, bias, bias_dtype, reinterpret_cast<uint8_t *>(Y), M, N, ldy, scale);
     return cudaGetLastError() == cudaSuccess ? GGUFB200_OK : GGUFB200_E_CUDA;
 }
 

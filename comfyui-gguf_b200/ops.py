@@ -23,7 +23,8 @@ import torch
 
 from . import _lib
 from ._host import comfy_lora, comfy_mm, comfy_ops
-from .dequant import FALLBACK_QTYPES, dequantize_fallback, dequantize_rows, dequantize_tensor, dtype_code, is_quantized, math_code
+from .dequant import (FALLBACK_QTYPES, dequantize, dequantize_fallback, dequantize_rows, dequantize_tensor, dtype_code, is_quantized,
+                      math_code)
 
 _Q = gguf.GGMLQuantizationType
 _FUSED_ACT = (torch.float16, torch.bfloat16)
@@ -158,9 +159,9 @@ LORA_KERNEL_MAX_RANK = 8 * LORA_MAX_RANK     # at most 8 LoRA k-blocks: a larger
 KRON_MAX_PATCHES = 8   # LoKr patches one ggufb200_dequant_kron call applies (csrc/internal.h kKronMaxPatches); more -> two-step route
 
 
-def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None):
+def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None, scale=None):
     """The call itself.  x: CUDA fp16/bf16 [..., K]; wraw: PLAIN uint8 tensor holding the packed rows on x.device;
-    bias: PLAIN tensor on x.device or None.  Kept free of tensor-subclass traffic (every attribute read on a GGMLTensor
+    bias: PLAIN tensor on x.device or None; scale (LoRA only): fp32 [N] feature scale of ggufb200_linear_lora_scaled.  Kept free of tensor-subclass traffic (every attribute read on a GGMLTensor
     goes through __torch_function__) and of per-call object construction: for short activations the host side of this
     function, not the GPU, bounds the layer."""
     x2 = x if x.dim() == 2 else x.reshape(-1, K)
@@ -192,7 +193,13 @@ def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None
         # T = x * down^T [M, 64 J] act dtype, U = scale * up [N, 64 J] fp16 (zero padded), per-tile k-block ranges or None
         t_pad, u_pad, tiles = lora
         J = u_pad.shape[1] // LORA_MAX_RANK
-        if J == 1 and tiles is None:
+        if scale is not None:
+            def call():
+                return L.ggufb200_linear_lora_scaled(qcode, w_ptr, None if spans is None else spans.data_ptr(), N, K, x2.data_ptr(), M,
+                                                     x2.stride(0), act, bias_ptr, bias_code, t_pad.data_ptr(), t_pad.stride(0), u_pad.data_ptr(),
+                                                     u_pad.stride(0), J, None if tiles is None else tiles.data_ptr(), scale.data_ptr(),
+                                                     y.data_ptr(), N, ws_ptr, need, algo, _current_stream_ptr(index))
+        elif J == 1 and tiles is None:
             def call():
                 return L.ggufb200_linear_lora(qcode, w_ptr, None if spans is None else spans.data_ptr(), N, K, x2.data_ptr(), M, x2.stride(0), act,
                                               bias_ptr, bias_code, t_pad.data_ptr(), t_pad.stride(0), u_pad.data_ptr(), y.data_ptr(), N, ws_ptr,
@@ -236,8 +243,9 @@ def linear_packed(x, weight, bias, dequant_dtype=None, algo=_lib.ALGO_AUTO, use_
                           math_code(dequant_dtype, x.dtype), algo, spans)
 
 
-def linear_dense(x, weight, bias=None):
-    """y = x @ weight.T + bias on the tensor-core GEMM with an already dense fp16/bf16 weight (ggufb200_gemm)."""
+def linear_dense(x, weight, bias=None, feature_scale=None):
+    """y = x @ weight.T + bias on the tensor-core GEMM with an already dense fp16/bf16 weight (ggufb200_gemm).
+    feature_scale: None, or a CUDA fp32 [N] tensor: y = feature_scale * (x @ weight.T) + bias (ggufb200_gemm_scaled)."""
     N, K = weight.shape
     x2 = x.reshape(-1, K)
     if x2.stride(-1) != 1 or (x2.stride(0) % 8) != 0 or (x2.data_ptr() % 16) != 0:
@@ -252,10 +260,30 @@ def linear_dense(x, weight, bias=None):
         bias = _plain(bias).contiguous()
         bias_ptr, bias_code = bias.data_ptr(), dtype_code(bias.dtype)
     with torch.cuda.device(x.device):
-        rc = _lib.lib().ggufb200_gemm(weight.data_ptr(), N, K, weight.stride(0), x2.data_ptr(), M, x2.stride(0), dtype_code(x.dtype),
-                                      bias_ptr, bias_code, y.data_ptr(), N, torch.cuda.current_stream(x.device).cuda_stream)
+        if feature_scale is None:
+            rc = _lib.lib().ggufb200_gemm(weight.data_ptr(), N, K, weight.stride(0), x2.data_ptr(), M, x2.stride(0), dtype_code(x.dtype),
+                                          bias_ptr, bias_code, y.data_ptr(), N, torch.cuda.current_stream(x.device).cuda_stream)
+        else:
+            rc = _lib.lib().ggufb200_gemm_scaled(weight.data_ptr(), N, K, weight.stride(0), x2.data_ptr(), M, x2.stride(0), dtype_code(x.dtype),
+                                                 bias_ptr, bias_code, feature_scale.data_ptr(), y.data_ptr(), N,
+                                                 torch.cuda.current_stream(x.device).cuda_stream)
     _lib.check(rc, f"ggufb200_gemm(M={M}, N={N}, K={K})")
     return y.reshape(*x.shape[:-1], N)
+
+
+def scale_columns(x, col_scale):
+    """act(fp32(x) * col_scale) for a CUDA fp16/bf16 x [..., K] and fp32 col_scale [K] (ggufb200_scale_columns), bit-identical to
+    `(x.float() * col_scale).to(x.dtype)`."""
+    K = x.shape[-1]
+    x2 = x.reshape(-1, K)
+    if x2.stride(-1) != 1 or (x2.stride(0) % 8) != 0 or (x2.data_ptr() % 16) != 0:
+        x2 = x2.contiguous()
+    y = torch.empty(x2.shape, dtype=x.dtype, device=x.device)
+    with torch.cuda.device(x.device):
+        rc = _lib.lib().ggufb200_scale_columns(x2.data_ptr(), x2.shape[0], K, x2.stride(0), dtype_code(x.dtype), col_scale.data_ptr(),
+                                               y.data_ptr(), K, torch.cuda.current_stream(x.device).cuda_stream)
+    _lib.check(rc, f"ggufb200_scale_columns(M={x2.shape[0]}, K={K})")
+    return y.reshape(x.shape)
 
 
 _BIG_EMBEDDING_ROWS = 64 * 1024     # loader threshold above which Embedding always takes the GGML load path (ops.py:116-117)
@@ -452,6 +480,176 @@ def lora_kernel_operands(terms, N, K, dtype, device):
                  for i in range(n_tiles)]
         tiles = torch.tensor(pairs, dtype=torch.int32).to(device)
     return down_pad, u_pad, tiles
+
+
+def dora_terms(patches):
+    """Recognise a patch list of whole-weight LoRA and LoHa entries of which at least one carries DoRA (`dora_scale`).
+
+    Entries follow comfy.lora's layout (see `lora_side_terms` and `lycoris_terms`).  Returns [(kind, strength, alpha, factors,
+    dora_scale), ...] in list order: kind "lora" with factors (up, down) and alpha = alpha / rank, or "loha" with factors (w1a,
+    w1b, w2a, w2b) and alpha = alpha / w1b.shape[0] (1.0 when alpha is None); dora_scale is the entry's tensor or None.  None when
+    the list has no DoRA entry (the other recognisers serve it) or when any entry needs the general machinery: strength_model
+    != 1, a function hook, an offset, LoCon mid weights, Tucker factors, reshape, factors that are not 2-D or do not chain, LoKr
+    or any other kind.  The dora_scale's axis is checked against the weight by `dora_axis`."""
+    def mat(t):
+        return torch.is_tensor(t) and t.dim() == 2
+
+    terms, any_dora = [], False
+    for entry in patches:
+        if len(entry) < 3 or entry[2] != 1.0 or any(extra is not None for extra in entry[3:5]):
+            return None
+        value = entry[1]
+        kind = {"LoRAAdapter": "lora", "LoHaAdapter": "loha"}.get(type(value).__name__)
+        if kind is not None and hasattr(value, "weights"):
+            payload = tuple(value.weights)
+        elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] in ("lora", "loha"):
+            kind, payload = value[0], tuple(value[1])
+        else:
+            return None
+        if kind == "lora":
+            if len(payload) < 2:
+                return None
+            up, down, alpha, mid, dora_scale, reshape = (payload + (None,) * 6)[:6]
+            if mid is not None or reshape is not None or not (mat(up) and mat(down)) or up.shape[1] != down.shape[0]:
+                return None
+            factors, rank = (up, down), down.shape[0]
+        else:
+            if len(payload) < 5:
+                return None
+            w1a, w1b, alpha, w2a, w2b, t1, t2, dora_scale = (payload + (None,) * 8)[:8]
+            if t1 is not None or t2 is not None or not all(mat(t) for t in (w1a, w1b, w2a, w2b)) or w1a.shape[1] != w1b.shape[0] \
+                    or w2a.shape[1] != w2b.shape[0] or w1a.shape[0] != w2a.shape[0] or w1b.shape[1] != w2b.shape[1]:
+                return None
+            factors, rank = (w1a, w1b, w2a, w2b), w1b.shape[0]
+        if dora_scale is not None:
+            if not torch.is_tensor(dora_scale):
+                return None
+            any_dora = True
+        terms.append((kind, float(entry[0]), 1.0 if alpha is None else float(alpha) / rank, factors, dora_scale))
+    return terms if any_dora else None
+
+
+def dora_axis(dora_scale, N, K):
+    """0 when `weight_decompose` normalises an [N, K] weight along the output axis (dora_scale [N, 1]: one norm per row, LyCORIS
+    wd_on_out), 1 along the input axis (dora_scale [1, K] or [K]: one norm per column), None for a shape whose reference
+    broadcast is not one factor per row or per column.  The reference picks the output axis when dora_scale.shape[0] == N."""
+    shape = tuple(dora_scale.shape)
+    if shape == (N, 1):
+        return 0
+    if shape in ((1, K), (K,)) and shape[0] != N:
+        return 1
+    return None
+
+
+def _dora_delta(kind, factors, device):
+    """The entry's fp32 delta as calculate_weight forms it: up @ down, or (w1a @ w1b) * (w2a @ w2b) for LoHa."""
+    f = [t.to(device=device, dtype=torch.float32) for t in factors]
+    if kind == "lora":
+        return torch.mm(f[0], f[1])
+    return torch.mm(f[0], f[1]) * torch.mm(f[2], f[3])
+
+
+def dora_replay(W, terms):
+    """The reference's calculate_weight over recognised `dora_terms` on W ([N, K] in the activation dtype, the dequantised weight;
+    not modified), in the same ops, dtype and device.  Returns each entry's DoRA factor s (W's dtype, [N] for the output axis,
+    [K] for the input axis; None for an entry without DoRA) and the patched weight.  Per entry with strength st and alpha a:
+        plain   W += ((st * a) * delta).to(W.dtype)
+        DoRA    Wc = W + (delta * a).to(W.dtype)
+                nrm = row norms of W (output axis: the weight BEFORE this patch) or column norms of Wc (input axis), + eps(W.dtype)
+                s = (fp32(dora_scale) / nrm).to(W.dtype);  Wc *= s
+                W = Wc if st == 1 else W + st * (Wc - W)"""
+    W = W.clone()
+    N, K = W.shape
+    eps = torch.finfo(W.dtype).eps
+    factors = []
+    for kind, strength, alpha, fac, dora_scale in terms:
+        delta = _dora_delta(kind, fac, W.device)
+        if dora_scale is None:
+            W += ((strength * alpha) * delta).to(W.dtype)
+            factors.append(None)
+            continue
+        delta *= alpha
+        Wc = W + delta.to(W.dtype)
+        if dora_scale.shape[0] == N:
+            nrm = W.reshape(N, -1).norm(dim=1, keepdim=True)
+        else:
+            nrm = Wc.transpose(0, 1).reshape(K, -1).norm(dim=1, keepdim=True).transpose(0, 1)
+        nrm = nrm + eps
+        s = (dora_scale.to(device=W.device, dtype=torch.float32) / nrm).to(W.dtype)
+        Wc *= s
+        if strength != 1.0:
+            Wc -= W
+            W += strength * Wc
+        else:
+            W = Wc
+        factors.append(s.reshape(-1))
+    return factors, W
+
+
+def dora_compact(terms, factors, N, K):
+    """The patched weight of `dora_replay` in the compact form
+        W_final = diag(r) W0 diag(c) + sum_j diag(rho_j) (a_j st_j up_j down_j) diag(gamma_j)
+    with the reference's factors s: a plain entry appends a term with rho = gamma = 1; an output-axis DoRA entry multiplies r
+    and every earlier rho_j by (1 - st + st s) and appends its term with rho = s; an input-axis entry does the same to c and
+    the gamma_j.  Returns r [N], c [K], [(a_j st_j, rho_j [N] or None, gamma_j [K] or None)] in float64 (None = ones)."""
+    dev = next(s.device for s in factors if s is not None)
+    r = torch.ones(N, dtype=torch.float64, device=dev)
+    c = torch.ones(K, dtype=torch.float64, device=dev)
+    rho, gamma, coef = [], [], []
+    for (_kind, strength, alpha, _fac, dora_scale), s in zip(terms, factors):
+        coef.append(strength * alpha)
+        if s is None:
+            rho.append(None)
+            gamma.append(None)
+            continue
+        s = s.double()
+        f = 1.0 - strength + strength * s
+        if dora_scale.shape[0] == N:
+            r *= f
+            rho = [f if p is None else p * f for p in rho] + [s]
+            gamma.append(None)
+        else:
+            c *= f
+            gamma = [f if g is None else g * f for g in gamma] + [s]
+            rho.append(None)
+    return r, c, list(zip(coef, rho, gamma))
+
+
+class DoraPlan:
+    """What a DoRA patch set costs per forward, built once (`build_dora_plan`):
+        r       fp32 [N] output feature scale (ggufb200_*_scaled)
+        c       fp32 [K] input feature scale (ggufb200_scale_columns) or None when no entry normalises the input axis
+        down    [R, K] activation dtype: the down'_j = down_j diag(gamma_j), stacked
+        up      [N, R] activation dtype: a_j st_j diag(rho_j) up_j, the side GEMMs' up-projection
+        kernel  (down_pad, u_pad) of ggufb200_linear_lora_scaled with U_j = a_j st_j diag(rho_j / r) up_j in fp16, or None when
+                R > LORA_KERNEL_MAX_RANK, some r_n == 0 or some rho_j / r is not finite in fp16 (then the side form serves)."""
+
+    def __init__(self, r, c, down, up, kernel):
+        self.r, self.c, self.down, self.up, self.kernel = r, c, down, up, kernel
+
+
+def build_dora_plan(W, terms, dtype):
+    """DoraPlan of recognised `dora_terms` (shapes checked) for the dequantised weight W ([N, K], `dtype`, on the device of the
+    forward)."""
+    N, K = W.shape
+    dev = W.device
+    factors, _patched = dora_replay(W, terms)
+    r, c, compact = dora_compact(terms, factors, N, K)
+    ups, downs = [], []
+    for (kind, _st, _a, fac, _ds), (coef, rho, gamma) in zip(terms, compact):
+        up, down = (fac[0].to(device=dev, dtype=torch.float32), fac[1].to(device=dev, dtype=torch.float32)) if kind == "lora" \
+            else loha_as_lora(*fac, dev)
+        ups.append(up.double() * (coef if rho is None else coef * rho[:, None]))
+        downs.append(down.double() if gamma is None else down.double() * gamma[None, :])
+    up = torch.cat(ups, 1)
+    down = torch.cat(downs, 0).to(dtype)
+    kernel = None
+    if down.shape[0] <= LORA_KERNEL_MAX_RANK and bool((r != 0).all()):
+        down_pad, u_pad, _tiles = lora_kernel_operands([(1.0, (up / r[:, None]).float(), down, None)], N, K, dtype, dev)
+        if bool(torch.isfinite(u_pad).all()):
+            kernel = (down_pad, u_pad)
+    has_c = any(g is not None for _coef, _rho, g in compact)            # some entry normalises the input axis
+    return DoraPlan(r.float(), c.float() if has_c else None, down, up.to(dtype), kernel)
 
 
 class GGMLLayer(torch.nn.Module):
@@ -725,6 +923,89 @@ class GGMLOps(comfy_ops.manual_cast):
             y2.addmm_(t, up_all.to(x2.dtype).t())
             return y
 
+        # DoRA (weight-decomposed LoRA, `dora_terms`): a list of whole-weight LoRA / LoHa entries with DoRA factors keeps the form
+        #   W_final = diag(r) W0 diag(c) + sum_j diag(rho_j) (a_j st_j up_j down_j) diag(gamma_j)
+        # (`dora_compact`; the factors are the reference's own, replayed once per patch set on the dequantised weight), so
+        #   y = r * ((x diag(c)) W0^T) + sum_j (x down'_j^T) (a_j st_j diag(rho_j) up_j)^T + b,   down'_j = down_j diag(gamma_j).
+        # In-kernel (the in-kernel LoRA's conditions): ggufb200_linear_lora_scaled with feature scale r and U_j = a_j st_j diag(rho_j / r)
+        # up_j.  Side form (everything else): the dequantised weight, ggufb200_gemm_scaled with r, plus the side GEMMs.
+        def _dora_terms(self):
+            """`dora_terms` of the weight's patch list with every factor and dora_scale shape checked against [N, K]; None -> two-step
+            route (also for lora_side_gemm = False and a patch_dtype other than None)."""
+            w = self.weight
+            if not self.lora_side_gemm or self.patch_dtype is not None:
+                return None
+            entries = []
+            for patch_list, _key in w.patches:
+                entries.extend(patch_list)
+            terms = dora_terms(entries)
+            if terms is None:
+                return None
+            N, K = tuple(w.tensor_shape)
+            for _kind, _st, _a, factors, dora_scale in terms:
+                if factors[0].shape[0] != N or factors[-1].shape[1] != K:
+                    return None
+                if dora_scale is not None and dora_axis(dora_scale, N, K) is None:
+                    return None
+            return terms
+
+        def _dense_weight(self, wraw, qtype, N, K, dtype):
+            """dequantize_tensor(weight, dtype, self.dequant_dtype) of the packed bytes `wraw` (on the forward's device): [N, K] in dtype."""
+            if qtype in FALLBACK_QTYPES:
+                return dequantize_fallback(wraw, qtype, (N, K), dtype)
+            if qtype == _Q.BF16 and dtype == torch.bfloat16:
+                return wraw.view(torch.bfloat16).view(N, K)
+            return dequantize(wraw, qtype, (N, K), dtype=dtype if self.dequant_dtype == "target" else self.dequant_dtype, out_dtype=dtype)
+
+        def _dora_plan(self, terms, src, wraw, qtype, N, K, dev, dtype):
+            """`build_dora_plan`, cached per patch set: identity + storage + version of every factor and dora_scale, the strengths,
+            the weight's storage, the device, the activation dtype and dequant_dtype (the factors s depend on all of them)."""
+            key = tuple((kind, st, a) + tuple(None if t is None else (id(t), t.data_ptr(), t._version, tuple(t.shape)) for t in factors + (ds,))
+                        for kind, st, a, factors, ds in terms) + (id(self.weight), src.data_ptr(), src._version, str(dev), dtype, self.dequant_dtype)
+            cached = self.__dict__.get("_gg_dora")
+            if cached is not None and cached[0] == key:
+                return cached[1]
+            plan = build_dora_plan(self._dense_weight(wraw, qtype, N, K, dtype), terms, dtype)
+            self.__dict__["_gg_dora"] = (key, plan)
+            return plan
+
+        def _dora_linear(self, input, terms):
+            """y for a DoRA patch list, or None (two-step route) for shapes the kernels do not take."""
+            w = self.weight
+            qtype, (N, K) = w.tensor_type, w.tensor_shape
+            if N % 8 or K % 8 or input.shape[-1] != K:
+                return None
+            dev, dtype = input.device, input.dtype
+            src = w.as_subclass(torch.Tensor)
+            resident = src.device == dev
+            wraw = src if resident else src.to(dev)
+            if not wraw.is_contiguous():
+                wraw = wraw.contiguous()
+            b = self.bias
+            if b is not None:
+                b = _plain(b)
+                if b.device != dev:
+                    b = b.to(dev)
+            plan = self._dora_plan(terms, src, wraw, qtype, N, K, dev, dtype)
+            x2 = input.reshape(-1, K)
+            M = x2.shape[0]
+            xs = x2 if plan.c is None else scale_columns(x2, plan.c)
+            math = math_code(self.dequant_dtype, dtype)
+            exact = (_lib.FLAG_EXACT_W if self.linear_numerics != "fast" else 0) | _lib.FLAG_W_STABLE
+            spans = None
+            if (self.repack_spans and resident and math == _F16_CODE and qtype != _Q.BF16 and qtype not in FALLBACK_QTYPES
+                    and needs_span_layout(qtype, K) and M > GEMV_MAX_M and not straddled_rows(qtype, K)):
+                spans = span_layout(w, wraw)
+            if (plan.kernel is not None and self.lora_in_kernel and math == _F16_CODE and qtype != _Q.BF16 and qtype not in FALLBACK_QTYPES
+                    and (spans is not None or not needs_span_layout(qtype, K))):
+                down_pad, u_pad = plan.kernel
+                t = linear_dense(x2, down_pad)                                     # T = x * down'^T, [M, 64 J]
+                y = _launch_linear(xs, wraw, qtype, N, K, b, math, _lib.ALGO_FUSED_TMEM | exact, spans, (t, u_pad, None), plan.r)
+            else:
+                y = linear_dense(xs, self._dense_weight(wraw, qtype, N, K, dtype), b, plan.r)
+                y.addmm_(x2 @ plan.down.t(), plan.up.t())
+            return y.reshape(*input.shape[:-1], N)
+
         def forward_ggml_cast_weights(self, input):
             fused = self._fused_ok(input)
             terms = self._lora_terms(input.device) if fused else None
@@ -785,6 +1066,12 @@ class GGMLOps(comfy_ops.manual_cast):
                         return y
                 if y is not None:
                     return self._add_lora(y, input, terms) if terms else y
+            elif fused and getattr(self.weight, "patches", None):
+                dora = self._dora_terms()                               # tried after the LoRA and LyCORIS recognisers declined
+                if dora is not None:
+                    y = self._dora_linear(input, dora)
+                    if y is not None:
+                        return y
             weight, bias = self.cast_bias_weight(input)
             return torch.nn.functional.linear(input, weight, bias)
 

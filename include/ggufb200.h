@@ -273,12 +273,38 @@ int ggufb200_linear_lora_ex(int ggml_type, const void *W_packed, const void *W_s
                             size_t workspace_bytes, int algo, void *stream);
 
 /*
+ * ggufb200_linear_lora_ex with a per-output-feature fp32 scale applied to the whole product before the bias:
+ *     Y = act(feature_scale[n] * (X * dequant(W)^T + T * U^T)[m, n] + bias[n])
+ * feature_scale: NULL (then this is ggufb200_linear_lora_ex, bit for bit) or N floats in device memory, 16-byte aligned
+ * (GGUFB200_E_ALIGN).  With split K the scale is applied once, to the summed fp32 partials.  The packed Linear uses it for
+ * DoRA patches: feature_scale holds the output-axis norm factors r, U carries rho_j / r so that T * U^T comes out right.
+ */
+int ggufb200_linear_lora_scaled(int ggml_type, const void *W_packed, const void *W_spans, int64_t N, int64_t K, const void *X, int64_t M,
+                                int64_t ldx, int act_dtype, const void *bias, int bias_dtype, const void *T, int64_t ldt, const void *U,
+                                int64_t ldu, int lora_kblocks, const int32_t *tile_kblocks, const float *feature_scale, void *Y,
+                                int64_t ldy, void *workspace, size_t workspace_bytes, int algo, void *stream);
+
+/*
  * Plain tensor-core GEMM on an already-dense weight: Y = X * W^T (+bias), W[N,K] in
  * act_dtype.  Used for the F16/BF16 (torch-compatible) Linears of a model and as the
  * second half of GGUFB200_ALGO_DEQUANT_MMA.
  */
 int ggufb200_gemm(const void *W, int64_t N, int64_t K, int64_t ldw, const void *X, int64_t M, int64_t ldx,
                   int act_dtype, const void *bias, int bias_dtype, void *Y, int64_t ldy, void *stream);
+
+/* ggufb200_gemm with a per-output-feature fp32 scale: Y = act(feature_scale[n] * (X * W^T)[m, n] + bias[n]).
+ * feature_scale: NULL (ggufb200_gemm, bit for bit) or N floats in device memory, 16-byte aligned (GGUFB200_E_ALIGN). */
+int ggufb200_gemm_scaled(const void *W, int64_t N, int64_t K, int64_t ldw, const void *X, int64_t M, int64_t ldx, int act_dtype,
+                         const void *bias, int bias_dtype, const float *feature_scale, void *Y, int64_t ldy, void *stream);
+
+/*
+ * Column scale: Y[m, k] = act(float(X[m, k]) * col_scale[k]) for m < M, k < K, one fp32 multiply and one round-to-nearest
+ * per element (bit-identical to torch's `(x.float() * c).to(x.dtype)`).  X, Y: act_dtype (0 fp16 / 1 bf16), row strides ldx /
+ * ldy in elements (>= K, multiples of 8), 16-byte aligned; col_scale: K floats in device memory, 16-byte aligned; K % 8 == 0.
+ * Y must not overlap X.  The packed Linear uses it for the input-axis factors of DoRA patches.
+ */
+int ggufb200_scale_columns(const void *X, int64_t M, int64_t K, int64_t ldx, int act_dtype, const float *col_scale, void *Y, int64_t ldy,
+                           void *stream);
 
 /* Diagnostics: the tiling a fused kernel uses for this problem when given `workspace_bytes` of scratch.
  * algo = GGUFB200_ALGO_FUSED_MMA (| flags): activation rows per tile (128), number of K ranges (1 = unsplit),
