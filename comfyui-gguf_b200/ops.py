@@ -298,14 +298,92 @@ def _collect_patches(tensor):
     return gathered, key
 
 
-def lora_side_terms(patches):
-    """Recognise a patch list that consists of plain LoRA deltas only (SURVEY 8f rank 1).
+def _patch_entries(tensor):
+    """`tensor.patches` ([(patch_list, key), ...]) flattened into one list of entries, where they are."""
+    return [entry for patch_list, _key in tensor.patches for entry in patch_list]
 
-    `patches` is the flat list `_collect_patches` returns; entries follow comfy.lora's layout
-    `(strength_patch, value, strength_model[, offset, function])` with value `("lora", (up, down, alpha, mid, dora_scale,
-    reshape))` or a LoRAAdapter object carrying the same tuple in `.weights`.  Returns [(scale, up[N, r], down[r, K]), ...]
-    with scale = strength_patch * alpha / r, or None when any entry needs the general `calculate_weight` machinery
-    (strength_model != 1, offset / function hooks, LoCon mid weights, DoRA, reshape, diff / loha / lokr ... patches)."""
+
+_ADAPTER_KINDS = {"LoRAAdapter": "lora", "LoHaAdapter": "loha", "LoKrAdapter": "lokr"}
+
+
+def _mat(t):
+    return torch.is_tensor(t) and t.dim() == 2
+
+
+def _decode_patch(entry, kinds=("lora", "loha", "lokr")):
+    """One comfy.lora patch entry `(strength_patch, value, strength_model[, offset, function])` of one of `kinds` as the record
+    (kind, strength, a, factors, band, dora_scale), or None when it needs the general `calculate_weight` machinery or is of
+    another kind.
+
+    The value is `(kind, payload)` or an adapter object carrying the payload in `.weights`, matched by its class name
+    (LoRAAdapter / LoHaAdapter / LoKrAdapter), not by type:
+        "lora"  (up, down, alpha, mid, dora_scale, reshape)               factors (up, down),  a = alpha / down.shape[0]
+        "loha"  (w1a, w1b, alpha, w2a, w2b, t1, t2, dora_scale)          factors (w1a, w1b, w2a, w2b),  a = alpha / w1b.shape[0]
+        "lokr"  (w1, w2, alpha, w1_a, w1_b, w2_a, w2_b, t2, dora_scale)  factors (w1, w2, w1_a, w1_b, w2_a, w2_b), w1 or (w1_a, w1_b)
+                given, likewise w2;  a = alpha / dim with dim = w1_b.shape[0] when w1 is decomposed, w2_b.shape[0] when w2 is
+                (that one wins), 1.0 when neither is
+    and a = 1.0 when alpha is None: comfy.lora.calculate_weight scales the delta by strength * a.  strength = float(strength_patch);
+    band = the offset (dim, start, size), dim 0 for output rows and 1 for input features, or None for the whole weight;
+    dora_scale = the entry's DoRA tensor or None.  None for strength_model != 1, a function hook, any other offset, LoCon mid,
+    reshape, Tucker factors (t1 / t2), a dora_scale that is not a tensor, and factors that are not 2-D or do not chain."""
+    if len(entry) < 3 or entry[2] != 1.0 or (len(entry) > 4 and entry[4] is not None):
+        return None
+    offset = entry[3] if len(entry) > 3 else None
+    band = None
+    if offset is not None:
+        if not isinstance(offset, (tuple, list)) or len(offset) != 3 or offset[0] not in (0, 1):
+            return None
+        band = (int(offset[0]), int(offset[1]), int(offset[2]))
+        if band[1] < 0 or band[2] <= 0:
+            return None
+    value = entry[1]
+    kind = _ADAPTER_KINDS.get(type(value).__name__)
+    if kind in kinds and hasattr(value, "weights"):
+        payload = tuple(value.weights)
+    elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] in kinds:
+        kind, payload = value[0], tuple(value[1])
+    else:
+        return None
+    if kind == "lora":
+        if len(payload) < 2:
+            return None
+        up, down, alpha, mid, dora_scale, reshape = (payload + (None,) * 4)[:6]
+        if mid is not None or reshape is not None or not (_mat(up) and _mat(down)) or up.shape[1] != down.shape[0]:
+            return None
+        factors, dim = (up, down), down.shape[0]
+    elif kind == "loha":
+        if len(payload) < 5:
+            return None
+        w1a, w1b, alpha, w2a, w2b, t1, t2, dora_scale = (payload + (None,) * 3)[:8]
+        if t1 is not None or t2 is not None or not all(_mat(t) for t in (w1a, w1b, w2a, w2b)) or w1a.shape[1] != w1b.shape[0] \
+                or w2a.shape[1] != w2b.shape[0] or w1a.shape[0] != w2a.shape[0] or w1b.shape[1] != w2b.shape[1]:
+            return None
+        factors, dim = (w1a, w1b, w2a, w2b), w1b.shape[0]
+    else:
+        if len(payload) < 7:
+            return None
+        w1, w2, alpha, w1_a, w1_b, w2_a, w2_b, t2, dora_scale = (payload + (None,) * 2)[:9]
+        if t2 is not None:
+            return None
+        dim = None
+        for whole, a, b in ((w1, w1_a, w1_b), (w2, w2_a, w2_b)):
+            if whole is not None:
+                if not _mat(whole):
+                    return None
+            elif _mat(a) and _mat(b) and a.shape[1] == b.shape[0]:
+                dim = b.shape[0]
+            else:
+                return None
+        factors = (w1, w2, w1_a, w1_b, w2_a, w2_b)
+    if dora_scale is not None and not torch.is_tensor(dora_scale):
+        return None
+    a = 1.0 if alpha is None or dim is None else float(alpha) / dim
+    return kind, float(entry[0]), a, factors, band, dora_scale
+
+
+def lora_side_terms(patches):
+    """Recognise a patch list of plain whole-weight LoRA deltas (SURVEY 8f rank 1): [(scale, up[N, r], down[r, K]), ...] with
+    scale = strength_patch * alpha / r, or None when any entry is anything else (`lora_band_terms` without offsets)."""
     terms = lora_band_terms(patches)
     if terms is None or any(band is not None for _s, _u, _d, band in terms):
         return None
@@ -313,106 +391,33 @@ def lora_side_terms(patches):
 
 
 def lora_band_terms(patches):
-    """`lora_side_terms` that also accepts an `offset = (dim, start, size)`: the LoRA patches the band `start .. start + size`
-    of the output rows (dim 0) or of the input features (dim 1) only.  ComfyUI gives diffusers-format LoRAs such offsets, one
-    entry per q / k / v / mlp slice of a fused Flux or SD3 weight.  Returns [(scale, up, down, band), ...] with band None
-    (the whole weight) or (dim, start, size), or None when any entry needs `calculate_weight` (as `lora_side_terms`)."""
+    """Recognise a patch list of plain LoRA entries, each on the whole weight or on a band (`_decode_patch`): ComfyUI gives
+    diffusers-format LoRAs an `offset = (dim, start, size)`, one entry per q / k / v / mlp slice of a fused Flux or SD3 weight,
+    and the LoRA then patches rows (dim 0) or input features (dim 1) `start .. start + size` only.  Returns [(scale, up, down,
+    band), ...] with scale = strength_patch * a, or None when any entry is not a plain LoRA (`lycoris_terms` of LoRA only)."""
     terms = []
     for entry in patches:
-        if len(entry) < 3 or entry[2] != 1.0 or (len(entry) > 4 and entry[4] is not None):
+        record = _decode_patch(entry, ("lora",))
+        if record is None or record[5] is not None:                            # not a plain LoRA
             return None
-        offset = entry[3] if len(entry) > 3 else None
-        band = None
-        if offset is not None:
-            if not isinstance(offset, (tuple, list)) or len(offset) != 3 or offset[0] not in (0, 1):
-                return None
-            band = (int(offset[0]), int(offset[1]), int(offset[2]))
-            if band[1] < 0 or band[2] <= 0:
-                return None
-        value = entry[1]
-        if type(value).__name__ == "LoRAAdapter" and hasattr(value, "weights"):
-            payload = value.weights
-        elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] == "lora":
-            payload = value[1]
-        else:
-            return None
-        up, down = payload[0], payload[1]
-        alpha = payload[2] if len(payload) > 2 else None
-        if any(extra is not None for extra in payload[3:6]):
-            return None
-        if not (torch.is_tensor(up) and torch.is_tensor(down)) or up.dim() != 2 or down.dim() != 2 or up.shape[1] != down.shape[0]:
-            return None
-        scale = float(entry[0]) * (1.0 if alpha is None else float(alpha) / down.shape[0])
-        terms.append((scale, up, down, band))
+        _kind, strength, a, (up, down), band, _dora_scale = record
+        terms.append((strength * a, up, down, band))
     return terms
 
 
 def lycoris_terms(patches):
-    """Recognise a patch list of LoRA, LoHa and LoKr (LyCORIS) entries, in any mix.
-
-    Entries follow comfy.lora's layout (see `lora_side_terms`); a LoHa value is `("loha", (w1a, w1b, alpha, w2a, w2b, t1, t2,
-    dora_scale))` or a LoHaAdapter carrying that tuple in `.weights`, a LoKr value `("lokr", (w1, w2, alpha, w1_a, w1_b, w2_a, w2_b,
-    t2, dora_scale))` or a LoKrAdapter.  Returns [(kind, scale, factors, band), ...] in list order:
-        "lora"  factors (up, down)                          scale as `lora_band_terms`
-        "loha"  factors (w1a, w1b, w2a, w2b)                scale = strength * alpha / w1b.shape[0] (strength when alpha is None)
-        "lokr"  factors (w1, w2, w1_a, w1_b, w2_a, w2_b),   w1 or (w1_a, w1_b) given, likewise w2;  scale = strength * alpha / dim
-                with dim = w1_b.shape[0] when w1 is decomposed, w2_b.shape[0] when w2 is (that one wins), strength when alpha is
-                None or neither is decomposed
-    which is how comfy.lora.calculate_weight scales them.  band as `lora_band_terms`.  None when any entry needs the general
-    machinery: strength_model != 1, a function hook, another offset, Tucker factors (t1 / t2), DoRA, factors that are not 2-D
-    or do not chain, any other patch kind."""
-    def mat(t):
-        return torch.is_tensor(t) and t.dim() == 2
-
+    """Recognise a patch list of LoRA, LoHa and LoKr (LyCORIS) entries without DoRA, in any mix (`_decode_patch`).  Returns
+    [(kind, scale, factors, band), ...] in list order with scale = strength_patch * a, or None when any entry needs
+    `calculate_weight`."""
     terms = []
     for entry in patches:
-        lora = lora_band_terms([entry])
-        if lora is not None:
-            scale, up, down, band = lora[0]
-            terms.append(("lora", scale, (up, down), band))
-            continue
-        if len(entry) < 3 or entry[2] != 1.0 or (len(entry) > 4 and entry[4] is not None):
+        record = _decode_patch(entry)
+        if record is None:
             return None
-        offset = entry[3] if len(entry) > 3 else None
-        band = None
-        if offset is not None:
-            if not isinstance(offset, (tuple, list)) or len(offset) != 3 or offset[0] not in (0, 1):
-                return None
-            band = (int(offset[0]), int(offset[1]), int(offset[2]))
-            if band[1] < 0 or band[2] <= 0:
-                return None
-        value = entry[1]
-        kind = {"LoHaAdapter": "loha", "LoKrAdapter": "lokr"}.get(type(value).__name__)
-        if kind is not None and hasattr(value, "weights"):
-            payload = value.weights
-        elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] in ("loha", "lokr"):
-            kind, payload = value
-        else:
+        kind, strength, a, factors, band, dora_scale = record
+        if dora_scale is not None:
             return None
-        strength = float(entry[0])
-        if kind == "loha":
-            if len(payload) < 5 or any(extra is not None for extra in payload[5:8]):
-                return None
-            w1a, w1b, alpha, w2a, w2b = payload[:5]
-            if not all(mat(t) for t in (w1a, w1b, w2a, w2b)) or w1a.shape[1] != w1b.shape[0] or w2a.shape[1] != w2b.shape[0] \
-                    or w1a.shape[0] != w2a.shape[0] or w1b.shape[1] != w2b.shape[1]:
-                return None
-            terms.append(("loha", strength * (1.0 if alpha is None else float(alpha) / w1b.shape[0]), (w1a, w1b, w2a, w2b), band))
-            continue
-        if len(payload) < 7 or any(extra is not None for extra in payload[7:9]):
-            return None
-        w1, w2, alpha, w1_a, w1_b, w2_a, w2_b = payload[:7]
-        dim = None
-        for whole, a, b in ((w1, w1_a, w1_b), (w2, w2_a, w2_b)):
-            if whole is not None:
-                if not mat(whole):
-                    return None
-            elif mat(a) and mat(b) and a.shape[1] == b.shape[0]:
-                dim = b.shape[0]
-            else:
-                return None
-        scale = strength * (float(alpha) / dim if alpha is not None and dim is not None else 1.0)
-        terms.append(("lokr", scale, (w1, w2, w1_a, w1_b, w2_a, w2_b), band))
+        terms.append((kind, strength * a, factors, band))
     return terms
 
 
@@ -443,6 +448,25 @@ def lokr_operands(factors, device):
     A = f32(w1) if w1 is not None else torch.mm(f32(w1_a), f32(w1_b))
     B = f32(w2) if w2 is not None else torch.mm(f32(w2_a), f32(w2_b))
     return A.contiguous(), B.contiguous()
+
+
+def lycoris_operands(terms, device):
+    """(LoRA terms, LoKr patches) of recognised `lycoris_terms` (shapes checked): LoRA entries as they are and LoHa entries as
+    LoRA terms of rank r1 r2 (`loha_as_lora`), all (scale, up, down, band); the LoKr entries as ((scale, A, B, band), ...) with
+    fp32 A / B on `device` (`lokr_operands`) and their ggufb200_kron_patch array, or None when there are none."""
+    lora, kron = [], []
+    for kind, scale, factors, band in terms:
+        if kind == "lora":
+            lora.append((scale, factors[0], factors[1], band))
+        elif kind == "loha":
+            lora.append((scale, *loha_as_lora(*factors, device), band))
+        else:
+            kron.append((scale, *lokr_operands(factors, device), band))
+    descs = (_lib.KronPatch * max(1, len(kron)))(*[
+        _lib.KronPatch(A.data_ptr(), B.data_ptr(), A.shape[0], A.shape[1], B.shape[0], B.shape[1], -1 if band is None else band[0],
+                       scale, 0 if band is None else band[1], 0 if band is None else band[2])
+        for scale, A, B, band in kron])
+    return lora, ((kron, descs) if kron else None)
 
 
 def lora_kernel_operands(terms, N, K, dtype, device):
@@ -483,50 +507,18 @@ def lora_kernel_operands(terms, N, K, dtype, device):
 
 
 def dora_terms(patches):
-    """Recognise a patch list of whole-weight LoRA and LoHa entries of which at least one carries DoRA (`dora_scale`).
-
-    Entries follow comfy.lora's layout (see `lora_side_terms` and `lycoris_terms`).  Returns [(kind, strength, alpha, factors,
-    dora_scale), ...] in list order: kind "lora" with factors (up, down) and alpha = alpha / rank, or "loha" with factors (w1a,
-    w1b, w2a, w2b) and alpha = alpha / w1b.shape[0] (1.0 when alpha is None); dora_scale is the entry's tensor or None.  None when
-    the list has no DoRA entry (the other recognisers serve it) or when any entry needs the general machinery: strength_model
-    != 1, a function hook, an offset, LoCon mid weights, Tucker factors, reshape, factors that are not 2-D or do not chain, LoKr
-    or any other kind.  The dora_scale's axis is checked against the weight by `dora_axis`."""
-    def mat(t):
-        return torch.is_tensor(t) and t.dim() == 2
-
-    terms, any_dora = [], False
+    """Recognise a patch list of whole-weight LoRA and LoHa entries of which at least one carries DoRA (`dora_scale`).  Returns
+    [(kind, strength, a, factors, dora_scale), ...] in list order (`_decode_patch`: a is kept apart from the strength, dora_scale
+    is None for a plain entry).  None when the list has no DoRA entry (the other recognisers serve it) or when any entry needs
+    `calculate_weight`, has an offset or is LoKr.  The dora_scale's axis is checked against the weight by `dora_axis`."""
+    terms = []
     for entry in patches:
-        if len(entry) < 3 or entry[2] != 1.0 or any(extra is not None for extra in entry[3:5]):
+        record = _decode_patch(entry, ("lora", "loha"))
+        if record is None or record[4] is not None:                            # banded DoRA is not served
             return None
-        value = entry[1]
-        kind = {"LoRAAdapter": "lora", "LoHaAdapter": "loha"}.get(type(value).__name__)
-        if kind is not None and hasattr(value, "weights"):
-            payload = tuple(value.weights)
-        elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] in ("lora", "loha"):
-            kind, payload = value[0], tuple(value[1])
-        else:
-            return None
-        if kind == "lora":
-            if len(payload) < 2:
-                return None
-            up, down, alpha, mid, dora_scale, reshape = (payload + (None,) * 6)[:6]
-            if mid is not None or reshape is not None or not (mat(up) and mat(down)) or up.shape[1] != down.shape[0]:
-                return None
-            factors, rank = (up, down), down.shape[0]
-        else:
-            if len(payload) < 5:
-                return None
-            w1a, w1b, alpha, w2a, w2b, t1, t2, dora_scale = (payload + (None,) * 8)[:8]
-            if t1 is not None or t2 is not None or not all(mat(t) for t in (w1a, w1b, w2a, w2b)) or w1a.shape[1] != w1b.shape[0] \
-                    or w2a.shape[1] != w2b.shape[0] or w1a.shape[0] != w2a.shape[0] or w1b.shape[1] != w2b.shape[1]:
-                return None
-            factors, rank = (w1a, w1b, w2a, w2b), w1b.shape[0]
-        if dora_scale is not None:
-            if not torch.is_tensor(dora_scale):
-                return None
-            any_dora = True
-        terms.append((kind, float(entry[0]), 1.0 if alpha is None else float(alpha) / rank, factors, dora_scale))
-    return terms if any_dora else None
+        kind, strength, a, factors, _band, dora_scale = record
+        terms.append((kind, strength, a, factors, dora_scale))
+    return terms if any(dora_scale is not None for *_t, dora_scale in terms) else None
 
 
 def dora_axis(dora_scale, N, K):
@@ -539,6 +531,37 @@ def dora_axis(dora_scale, N, K):
     if shape in ((1, K), (K,)) and shape[0] != N:
         return 1
     return None
+
+
+def _fits_weight(kind, factors, band, N, K):
+    """True when a recognised term's delta has the shape of its band of an [N, K] weight (the whole weight for band None) and
+    the band lies inside the weight: LoRA / LoHa rows from factors[0] and columns from factors[-1], LoKr a1 b1 x a2 b2."""
+    rows, cols = N, K
+    if band is not None:
+        dim, start, size = band
+        if start + size > (N, K)[dim]:
+            return False
+        rows, cols = (size, K) if dim == 0 else (N, size)
+    if kind == "lokr":
+        (a1, a2), (b1, b2) = lokr_factor_shapes(factors)
+        return a1 * b1 == rows and a2 * b2 == cols
+    return factors[0].shape[0] == rows and factors[-1].shape[1] == cols
+
+
+def _tensor_key(t):
+    """Identity, storage, version and shape of a patch factor (None for an absent one): a factor that was swapped for another
+    one (even at a recycled id()) or modified in place changes the key of every plan built from it."""
+    return None if t is None else (id(t), t.data_ptr(), t._version, tuple(t.shape))
+
+
+def _cached(owner, slot, key, build):
+    """`owner.__dict__[slot]` holds (key, value): the value when its key equals `key`, else `build()`, stored with `key`."""
+    cached = owner.__dict__.get(slot)
+    if cached is not None and cached[0] == key:
+        return cached[1]
+    value = build()
+    owner.__dict__[slot] = (key, value)
+    return value
 
 
 def _dora_delta(kind, factors, device):
@@ -796,22 +819,10 @@ class GGMLOps(comfy_ops.manual_cast):
                 return []
             if not self.lora_side_gemm or self.patch_dtype not in (None, "target"):
                 return None
-            entries = []
-            for patch_list, _key in w.patches:
-                entries.extend(patch_list)
-            terms = lora_band_terms(entries)
-            if terms is None:
-                return None
+            terms = lora_band_terms(_patch_entries(w))
             N, K = tuple(w.tensor_shape)
-            for _s, up, down, band in terms:
-                rows, cols = N, K
-                if band is not None:
-                    dim, start, size = band
-                    if start + size > (N, K)[dim]:
-                        return None
-                    rows, cols = (size, K) if dim == 0 else (N, size)
-                if tuple(up.shape) != (rows, down.shape[0]) or down.shape[1] != cols:
-                    return None
+            if terms is None or not all(_fits_weight("lora", (up, down), band, N, K) for _s, up, down, band in terms):
+                return None
             return terms
 
         # LoRA inside the fused kernel (GGUFB200_ALGO_FUSED_TMEM, csrc/linear_sm90.cu: J <= 8 extra k-blocks, SURVEY 8f rank 1):
@@ -822,69 +833,23 @@ class GGMLOps(comfy_ops.manual_cast):
         lora_in_kernel = True
 
         def _lora_operands(self, terms, dev, dtype):
-            # identity + storage + version of every factor: a patch set that was swapped for another one (even at a recycled
-            # id()) or modified in place rebuilds the operands
-            key = tuple((id(up), up.data_ptr(), up._version, tuple(up.shape), id(down), down.data_ptr(), down._version, float(scale), band)
-                        for scale, up, down, band in terms) + (str(dev), dtype)
-            cached = self.__dict__.get("_gg_lora")
-            if cached is not None and cached[0] == key:
-                return cached[1]
-            N, K = tuple(self.weight.tensor_shape)
-            operands = lora_kernel_operands(terms, N, K, dtype, dev)
-            self.__dict__["_gg_lora"] = (key, operands)
-            return operands
+            """`lora_kernel_operands` of `_lora_terms`, cached per patch set, device and activation dtype."""
+            key = tuple((float(scale), band, _tensor_key(up), _tensor_key(down)) for scale, up, down, band in terms) + (str(dev), dtype)
+            return _cached(self, "_gg_lora", key, lambda: lora_kernel_operands(terms, *self.weight.tensor_shape, dtype, dev))
 
         def _lycoris_terms(self, dev):
-            """For a patch list with LoHa / LoKr entries (`lycoris_terms`, any mix with LoRA): (LoRA terms, LoKr patches) with the
-            LoHa entries as LoRA terms of rank r1 r2 and each LoKr entry as (scale, A, B, band), fp32 A / B on `dev`; both built
-            once per patch set.  None -> two-step route (also for patch_dtype other than None: the reference then forms the
-            delta in another dtype)."""
+            """For a patch list with LoHa / LoKr entries (`lycoris_terms`, any mix with LoRA): `lycoris_operands` on `dev`, cached
+            per patch set.  None -> two-step route (also for patch_dtype other than None: the reference then forms the delta in
+            another dtype)."""
             w = self.weight
             if not self.lora_side_gemm or self.patch_dtype is not None:
                 return None
-            entries = []
-            for patch_list, _key in w.patches:
-                entries.extend(patch_list)
-            terms = lycoris_terms(entries)
-            if terms is None:
-                return None
+            terms = lycoris_terms(_patch_entries(w))
             N, K = tuple(w.tensor_shape)
-            for kind, _s, factors, band in terms:
-                rows, cols = N, K
-                if band is not None:
-                    dim, start, size = band
-                    if start + size > (N, K)[dim]:
-                        return None
-                    rows, cols = (size, K) if dim == 0 else (N, size)
-                if kind == "lokr":
-                    (a1, a2), (b1, b2) = lokr_factor_shapes(factors)
-                    if a1 * b1 != rows or a2 * b2 != cols:
-                        return None
-                else:
-                    up, down = factors[0], factors[-1]      # LoRA (up, down); LoHa: w1a and w2b carry the shape
-                    if up.shape[0] != rows or down.shape[1] != cols:
-                        return None
-            # identity + storage + version of every factor, as for `_lora_operands`
-            key = tuple((kind, float(scale), band) + tuple((id(t), t.data_ptr(), t._version, tuple(t.shape)) if t is not None else None
-                                                            for t in factors) for kind, scale, factors, band in terms) + (str(dev),)
-            cached = self.__dict__.get("_gg_lycoris")
-            if cached is not None and cached[0] == key:
-                return cached[1]
-            lora, kron = [], []
-            for kind, scale, factors, band in terms:
-                if kind == "lora":
-                    lora.append((scale, factors[0], factors[1], band))
-                elif kind == "loha":
-                    lora.append((scale, *loha_as_lora(*factors, dev), band))
-                else:
-                    kron.append((scale, *lokr_operands(factors, dev), band))
-            descs = (_lib.KronPatch * max(1, len(kron)))(*[
-                _lib.KronPatch(A.data_ptr(), B.data_ptr(), A.shape[0], A.shape[1], B.shape[0], B.shape[1], -1 if band is None else band[0],
-                               scale, 0 if band is None else band[1], 0 if band is None else band[2])
-                for scale, A, B, band in kron])
-            operands = (lora, (kron, descs) if kron else None)
-            self.__dict__["_gg_lycoris"] = (key, operands)
-            return operands
+            if terms is None or not all(_fits_weight(kind, factors, band, N, K) for kind, _s, factors, band in terms):
+                return None
+            key = tuple((kind, float(scale), band) + tuple(map(_tensor_key, factors)) for kind, scale, factors, band in terms) + (str(dev),)
+            return _cached(self, "_gg_lycoris", key, lambda: lycoris_operands(terms, dev))
 
         def _kron_linear(self, input, wraw, qtype, N, K, bias, kron):
             """ggufb200_dequant_kron (the patched weight, bit-identical to the reference's) into an [N, K] workspace, then
@@ -927,7 +892,7 @@ class GGMLOps(comfy_ops.manual_cast):
         #   W_final = diag(r) W0 diag(c) + sum_j diag(rho_j) (a_j st_j up_j down_j) diag(gamma_j)
         # (`dora_compact`; the factors are the reference's own, replayed once per patch set on the dequantised weight), so
         #   y = r * ((x diag(c)) W0^T) + sum_j (x down'_j^T) (a_j st_j diag(rho_j) up_j)^T + b,   down'_j = down_j diag(gamma_j).
-        # In-kernel (the in-kernel LoRA's conditions): ggufb200_linear_lora_scaled with feature scale r and U_j = a_j st_j diag(rho_j / r)
+        # In-kernel (`_takes_lora_kblocks`): ggufb200_linear_lora_scaled with feature scale r and U_j = a_j st_j diag(rho_j / r)
         # up_j.  Side form (everything else): the dequantised weight, ggufb200_gemm_scaled with r, plus the side GEMMs.
         def _dora_terms(self):
             """`dora_terms` of the weight's patch list with every factor and dora_scale shape checked against [N, K]; None -> two-step
@@ -935,18 +900,11 @@ class GGMLOps(comfy_ops.manual_cast):
             w = self.weight
             if not self.lora_side_gemm or self.patch_dtype is not None:
                 return None
-            entries = []
-            for patch_list, _key in w.patches:
-                entries.extend(patch_list)
-            terms = dora_terms(entries)
-            if terms is None:
-                return None
+            terms = dora_terms(_patch_entries(w))
             N, K = tuple(w.tensor_shape)
-            for _kind, _st, _a, factors, dora_scale in terms:
-                if factors[0].shape[0] != N or factors[-1].shape[1] != K:
-                    return None
-                if dora_scale is not None and dora_axis(dora_scale, N, K) is None:
-                    return None
+            if terms is None or not all(_fits_weight(kind, factors, None, N, K) and (ds is None or dora_axis(ds, N, K) is not None)
+                                        for kind, _st, _a, factors, ds in terms):
+                return None
             return terms
 
         def _dense_weight(self, wraw, qtype, N, K, dtype):
@@ -960,118 +918,108 @@ class GGMLOps(comfy_ops.manual_cast):
         def _dora_plan(self, terms, src, wraw, qtype, N, K, dev, dtype):
             """`build_dora_plan`, cached per patch set: identity + storage + version of every factor and dora_scale, the strengths,
             the weight's storage, the device, the activation dtype and dequant_dtype (the factors s depend on all of them)."""
-            key = tuple((kind, st, a) + tuple(None if t is None else (id(t), t.data_ptr(), t._version, tuple(t.shape)) for t in factors + (ds,))
-                        for kind, st, a, factors, ds in terms) + (id(self.weight), src.data_ptr(), src._version, str(dev), dtype, self.dequant_dtype)
-            cached = self.__dict__.get("_gg_dora")
-            if cached is not None and cached[0] == key:
-                return cached[1]
-            plan = build_dora_plan(self._dense_weight(wraw, qtype, N, K, dtype), terms, dtype)
-            self.__dict__["_gg_dora"] = (key, plan)
-            return plan
+            key = tuple((kind, st, a) + tuple(map(_tensor_key, factors + (ds,))) for kind, st, a, factors, ds in terms) \
+                + (id(self.weight), src.data_ptr(), src._version, str(dev), dtype, self.dequant_dtype)
+            return _cached(self, "_gg_dora", key, lambda: build_dora_plan(self._dense_weight(wraw, qtype, N, K, dtype), terms, dtype))
 
-        def _dora_linear(self, input, terms):
-            """y for a DoRA patch list, or None (two-step route) for shapes the kernels do not take."""
+        def _dora_linear(self, input, terms, src, wraw, resident, bias, M):
+            """y for a DoRA patch list (`_dora_terms`) on a weight with N and K multiples of 8; the other arguments as
+            `forward_ggml_cast_weights` prepares them."""
             w = self.weight
             qtype, (N, K) = w.tensor_type, w.tensor_shape
-            if N % 8 or K % 8 or input.shape[-1] != K:
-                return None
             dev, dtype = input.device, input.dtype
-            src = w.as_subclass(torch.Tensor)
-            resident = src.device == dev
-            wraw = src if resident else src.to(dev)
             if not wraw.is_contiguous():
                 wraw = wraw.contiguous()
-            b = self.bias
-            if b is not None:
-                b = _plain(b)
-                if b.device != dev:
-                    b = b.to(dev)
             plan = self._dora_plan(terms, src, wraw, qtype, N, K, dev, dtype)
             x2 = input.reshape(-1, K)
-            M = x2.shape[0]
             xs = x2 if plan.c is None else scale_columns(x2, plan.c)
             math = math_code(self.dequant_dtype, dtype)
             exact = (_lib.FLAG_EXACT_W if self.linear_numerics != "fast" else 0) | _lib.FLAG_W_STABLE
-            spans = None
-            if (self.repack_spans and resident and math == _F16_CODE and qtype != _Q.BF16 and qtype not in FALLBACK_QTYPES
-                    and needs_span_layout(qtype, K) and M > GEMV_MAX_M and not straddled_rows(qtype, K)):
-                spans = span_layout(w, wraw)
-            if (plan.kernel is not None and self.lora_in_kernel and math == _F16_CODE and qtype != _Q.BF16 and qtype not in FALLBACK_QTYPES
-                    and (spans is not None or not needs_span_layout(qtype, K))):
+            spans = span_layout(w, wraw) if self._takes_span_copy(qtype, N, K, M, math, resident) else None
+            if plan.kernel is not None and self._takes_lora_kblocks(qtype, N, K, math, spans):
                 down_pad, u_pad = plan.kernel
                 t = linear_dense(x2, down_pad)                                     # T = x * down'^T, [M, 64 J]
-                y = _launch_linear(xs, wraw, qtype, N, K, b, math, _lib.ALGO_FUSED_TMEM | exact, spans, (t, u_pad, None), plan.r)
+                y = _launch_linear(xs, wraw, qtype, N, K, bias, math, _lib.ALGO_FUSED_TMEM | exact, spans, (t, u_pad, None), plan.r)
             else:
-                y = linear_dense(xs, self._dense_weight(wraw, qtype, N, K, dtype), b, plan.r)
+                y = linear_dense(xs, self._dense_weight(wraw, qtype, N, K, dtype), bias, plan.r)
                 y.addmm_(x2 @ plan.down.t(), plan.up.t())
             return y.reshape(*input.shape[:-1], N)
 
+        def _takes_span_copy(self, qtype, N, K, M, math, resident):
+            """True when the FUSED_TMEM kernel reads the re-packed span-major copy of the weight (`span_layout`): the canonical
+            rows cannot be staged by TMA and the copy is allowed, resident, and worth it at this M."""
+            return (self.repack_spans and resident and M > GEMV_MAX_M and math == _F16_CODE and N % 8 == 0 and qtype != _Q.BF16
+                    and needs_span_layout(qtype, K) and qtype not in FALLBACK_QTYPES and not straddled_rows(qtype, K))
+
+        def _takes_lora_kblocks(self, qtype, N, K, math, spans):
+            """True when the FUSED_TMEM kernel may run LoRA k-blocks on this weight (`lora_in_kernel`); the caller adds its rank
+            limit.  `spans`: the span copy the forward reads, or None."""
+            return (self.lora_in_kernel and math == _F16_CODE and N % 8 == 0 and qtype != _Q.BF16 and qtype not in FALLBACK_QTYPES
+                    and (spans is not None or not needs_span_layout(qtype, K)))
+
         def forward_ggml_cast_weights(self, input):
-            fused = self._fused_ok(input)
-            terms = self._lora_terms(input.device) if fused else None
-            kron = None
-            if terms is None and fused and getattr(self.weight, "patches", None) and self.weight.tensor_type not in FALLBACK_QTYPES:
-                lycoris = self._lycoris_terms(input.device)           # LoHa / LoKr entries: LoRA terms + LoKr patches
-                if lycoris is not None:
-                    terms, kron = lycoris
-            if terms is not None:
+            y = None
+            if self._fused_ok(input):
                 dev = input.device
-                w = self.weight
-                qtype, (N, K) = w.tensor_type, w.tensor_shape          # plain Python attributes: no subclass dispatch
-                wraw = w.as_subclass(torch.Tensor)
-                resident = wraw.device == dev
-                if not resident:
-                    wraw = wraw.to(dev)                                # offloaded module: packed bytes H2D
-                b = self.bias
-                if b is not None:
-                    b = _plain(b)
-                    if b.device != dev:
-                        b = b.to(dev)
-                M = input.numel() // K if input.shape[-1] == K else -1
-                y = None
-                if M < 0:
-                    pass                                               # feature mismatch: let F.linear raise the usual error
-                elif qtype in FALLBACK_QTYPES:
-                    # numpy-fallback types (csrc/fallback.cuh): no fused kernel reads them, so K1 into an [N, K] activation-dtype
-                    # weight (the reference's fp32 -> dtype rounding) + the dense GEMM at every M; other shapes: two-step route
-                    if N % 8 == 0 and K % 8 == 0:
-                        W = dequantize_fallback(wraw, qtype, (N, K), input.dtype)
-                        y = linear_dense(input, W, b)
-                elif kron is not None:
-                    # LoKr: the patched weight in one K1 launch + the dense GEMM at every M; LoRA / LoHa terms as side GEMMs
-                    if qtype != _Q.BF16 and N % 8 == 0 and K % 8 == 0 and len(kron[0]) <= KRON_MAX_PATCHES:
-                        y = self._kron_linear(input, wraw, qtype, N, K, b, kron)
-                elif qtype == _Q.BF16 and M > GEMV_MAX_M:
-                    if input.dtype == torch.bfloat16 and K % 8 == 0 and N % 8 == 0:   # already dense: straight to the tensor-core GEMM
-                        y = linear_dense(input, wraw.view(torch.bfloat16).view(N, K), b)
-                elif M <= GEMV_MAX_M or N % 8 == 0:                    # (the M <= 8 kernel stores per element: any N)
-                    math = math_code(self.dequant_dtype, input.dtype)
-                    algo, spans = _lib.ALGO_AUTO, None
-                    # W_STABLE: the packed weight is a parameter (or its host-to-device copy just above): never written by a kernel in flight
-                    exact = (_lib.FLAG_EXACT_W if self.linear_numerics != "fast" else 0) | _lib.FLAG_W_STABLE
-                    algo |= exact
-                    if (self.repack_spans and resident and math == _F16_CODE and N % 8 == 0 and qtype != _Q.BF16
-                            and needs_span_layout(qtype, K) and M > GEMV_MAX_M and not straddled_rows(qtype, K)):
-                        spans = span_layout(w, wraw)                   # cached on the tensor after the first forward
-                        algo = _lib.ALGO_FUSED_TMEM | exact
-                    lora = None
-                    if (terms and self.lora_in_kernel and math == _F16_CODE and N % 8 == 0
-                            and qtype != _Q.BF16 and sum(d.shape[0] for _s, _u, d, _b in terms) <= LORA_KERNEL_MAX_RANK
-                            and (spans is not None or not needs_span_layout(qtype, K))):
-                        down_pad, u_pad, tiles = self._lora_operands(terms, dev, input.dtype)
-                        lora = (linear_dense(input.reshape(-1, K), down_pad), u_pad, tiles)       # T = x * down^T, [M, 64 J]
-                        algo = _lib.ALGO_FUSED_TMEM | exact
-                    y = _launch_linear(input, wraw, qtype, N, K, b, math, algo, spans, lora)
-                    if lora is not None:
-                        return y
-                if y is not None:
-                    return self._add_lora(y, input, terms) if terms else y
-            elif fused and getattr(self.weight, "patches", None):
-                dora = self._dora_terms()                               # tried after the LoRA and LyCORIS recognisers declined
-                if dora is not None:
-                    y = self._dora_linear(input, dora)
-                    if y is not None:
-                        return y
+                terms, kron, dora = self._lora_terms(dev), None, None
+                if terms is None and self.weight.tensor_type not in FALLBACK_QTYPES:
+                    lycoris = self._lycoris_terms(dev)                 # LoHa / LoKr entries: LoRA terms + LoKr patches
+                    if lycoris is not None:
+                        terms, kron = lycoris
+                if terms is None:
+                    dora = self._dora_terms()                          # tried after the LoRA and LyCORIS recognisers declined
+                if terms is not None or dora is not None:
+                    w = self.weight
+                    qtype, (N, K) = w.tensor_type, w.tensor_shape      # plain Python attributes: no subclass dispatch
+                    src = w.as_subclass(torch.Tensor)
+                    resident = src.device == dev
+                    wraw = src if resident else src.to(dev)            # offloaded module: packed bytes H2D
+                    b = self.bias
+                    if b is not None:
+                        b = _plain(b)
+                        if b.device != dev:
+                            b = b.to(dev)
+                    M = input.numel() // K if input.shape[-1] == K else -1
+                    if M < 0:
+                        pass                                           # feature mismatch: let F.linear raise the usual error
+                    elif dora is not None:
+                        if N % 8 == 0 and K % 8 == 0:
+                            y = self._dora_linear(input, dora, src, wraw, resident, b, M)
+                    elif qtype in FALLBACK_QTYPES:
+                        # numpy-fallback types (csrc/fallback.cuh): no fused kernel reads them, so K1 into an [N, K] activation-dtype
+                        # weight (the reference's fp32 -> dtype rounding) + the dense GEMM at every M; other shapes: two-step route
+                        if N % 8 == 0 and K % 8 == 0:
+                            W = dequantize_fallback(wraw, qtype, (N, K), input.dtype)
+                            y = linear_dense(input, W, b)
+                    elif kron is not None:
+                        # LoKr: the patched weight in one K1 launch + the dense GEMM at every M; LoRA / LoHa terms as side GEMMs
+                        if qtype != _Q.BF16 and N % 8 == 0 and K % 8 == 0 and len(kron[0]) <= KRON_MAX_PATCHES:
+                            y = self._kron_linear(input, wraw, qtype, N, K, b, kron)
+                    elif qtype == _Q.BF16 and M > GEMV_MAX_M:
+                        if input.dtype == torch.bfloat16 and K % 8 == 0 and N % 8 == 0:   # already dense: straight to the tensor-core GEMM
+                            y = linear_dense(input, wraw.view(torch.bfloat16).view(N, K), b)
+                    elif M <= GEMV_MAX_M or N % 8 == 0:                # (the M <= 8 kernel stores per element: any N)
+                        math = math_code(self.dequant_dtype, input.dtype)
+                        # W_STABLE: the packed weight is a parameter (or its host-to-device copy just above): never written by a
+                        # kernel in flight
+                        exact = (_lib.FLAG_EXACT_W if self.linear_numerics != "fast" else 0) | _lib.FLAG_W_STABLE
+                        algo, spans = _lib.ALGO_AUTO | exact, None
+                        if self._takes_span_copy(qtype, N, K, M, math, resident):
+                            spans = span_layout(w, wraw)               # cached on the tensor after the first forward
+                            algo = _lib.ALGO_FUSED_TMEM | exact
+                        lora = None
+                        if (terms and self._takes_lora_kblocks(qtype, N, K, math, spans)
+                                and sum(d.shape[0] for _s, _u, d, _b in terms) <= LORA_KERNEL_MAX_RANK):
+                            down_pad, u_pad, tiles = self._lora_operands(terms, dev, input.dtype)
+                            lora = (linear_dense(input.reshape(-1, K), down_pad), u_pad, tiles)       # T = x * down^T, [M, 64 J]
+                            algo = _lib.ALGO_FUSED_TMEM | exact
+                        y = _launch_linear(input, wraw, qtype, N, K, b, math, algo, spans, lora)
+                        if lora is not None:
+                            return y
+                    if y is not None and terms:
+                        y = self._add_lora(y, input, terms)
+            if y is not None:
+                return y
             weight, bias = self.cast_bias_weight(input)
             return torch.nn.functional.linear(input, weight, bias)
 
