@@ -26,6 +26,11 @@ int rows_dispatch(int type, const void *packed, long long n_table_rows, long lon
 constexpr int kKronMaxPatches = 8;
 int dequant_kron_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
                           const ggufb200_kron_patch *patches, int n_patches, cudaStream_t st, bool stable);
+// lowrank.cu, ggufb200_dequant_lowrank: the [N, K] weight (flat block stream, K % 32 == 0) with LoRA / LoHa patches applied;
+// block formats and fallback formats; `patches` validated by the caller (api.cu)
+constexpr int kLowrankMaxPatches = GGUFB200_LOWRANK_MAX_PATCHES;
+int dequant_lowrank_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
+                             const ggufb200_lowrank_patch *patches, int n_patches, cudaStream_t st);
 
 // ------------------------------------------------------------------ small-M Linear: gemv.cu (GGUFB200_ALGO_GEMV), gemv2.cu (GEMV_FAST)
 int gemv_max_m();

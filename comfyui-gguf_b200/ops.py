@@ -23,8 +23,8 @@ import torch
 
 from . import _lib
 from ._host import comfy_lora, comfy_mm, comfy_ops
-from .dequant import (FALLBACK_QTYPES, dequantize, dequantize_fallback, dequantize_rows, dequantize_tensor, dtype_code, is_quantized,
-                      math_code)
+from .dequant import (FALLBACK_QTYPES, SUPPORTED_QTYPES, dequantize, dequantize_fallback, dequantize_rows, dequantize_tensor, dtype_code,
+                      is_quantized, math_code)
 
 _Q = gguf.GGMLQuantizationType
 _FUSED_ACT = (torch.float16, torch.bfloat16)
@@ -157,6 +157,9 @@ def span_layout(weight, wraw):
 LORA_MAX_RANK = 64     # width of one LoRA k-block of the FUSED_TMEM kernel
 LORA_KERNEL_MAX_RANK = 8 * LORA_MAX_RANK     # at most 8 LoRA k-blocks: a larger total rank takes the side GEMMs (`_add_lora`)
 KRON_MAX_PATCHES = 8   # LoKr patches one ggufb200_dequant_kron call applies (csrc/internal.h kKronMaxPatches); more -> two-step route
+# weight types and activation dtypes ggufb200_dequant_lowrank serves (every block format and numpy-fallback type but BF16)
+_LOWRANK_QTYPES = tuple(q for q in SUPPORTED_QTYPES if q != _Q.BF16) + FALLBACK_QTYPES
+_LOWRANK_ACT = (torch.float16, torch.bfloat16, torch.float32)
 
 
 def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None, scale=None):
@@ -419,6 +422,72 @@ def lycoris_terms(patches):
             return None
         terms.append((kind, strength * a, factors, band))
     return terms
+
+
+def _flat_lora_entry(entry):
+    """(entry', sources): `entry` with the up / down factors of a LoRA / LoCon payload flattened to 2-D as calculate_weight
+    multiplies them (`flatten(start_dim=1)`: up [Cout, r, 1, 1] -> [Cout, r], down [r, Cin, kh, kw] -> [r, Cin kh kw]) and the
+    two 4-D tensors it flattened; (entry, None) for any other entry.  LoHa factors are not flattened: the reference multiplies
+    them with torch.mm as they come."""
+    value = entry[1] if len(entry) > 1 else None
+    if _ADAPTER_KINDS.get(type(value).__name__) == "lora" and hasattr(value, "weights"):
+        payload = tuple(value.weights)
+    elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] == "lora":
+        payload = tuple(value[1])
+    else:
+        return entry, None
+    if len(payload) < 2 or not all(torch.is_tensor(t) and t.dim() == 4 for t in payload[:2]):
+        return entry, None
+    flat = (entry[0], ("lora", tuple(t.flatten(start_dim=1) for t in payload[:2]) + payload[2:])) + tuple(entry[2:])
+    return flat, payload[:2]
+
+
+def conv_patch_terms(patches):
+    """Recognise a Conv2d patch list of whole-weight LoRA / LoCon and LoHa entries (`_decode_patch`, LoRA factors flattened by
+    `_flat_lora_entry`).  Returns [(kind, scale, factors, sources), ...] in list order with scale = strength_patch * a, factors
+    the 2-D matrices of the delta ((up, down) or (w1a, w1b, w2a, w2b)) and sources the entry's own tensors (cache keys), or None
+    when any entry is LoKr, has an offset, carries DoRA or needs `calculate_weight` (strength_model != 1, a hook, Tucker / mid,
+    reshape).  The Linear recognisers are separate and keep refusing 4-D factors."""
+    terms = []
+    for entry in patches:
+        flat, sources = _flat_lora_entry(entry)
+        record = _decode_patch(flat, ("lora", "loha"))
+        if record is None or record[4] is not None or record[5] is not None:
+            return None
+        kind, strength, a, factors, _band, _dora_scale = record
+        terms.append((kind, strength * a, factors, factors if sources is None else sources))
+    return terms
+
+
+def lowrank_pays(N, K, terms):
+    """True when ggufb200_dequant_lowrank is expected to form the patched [N, K] weight faster than the two-step route (K1 +
+    calculate_weight).  Cost model in microseconds, fitted to tools/bench_conv_patches.py on an NVIDIA H100 80GB HBM3 at 700 W
+    (Q4_K, fp16, SD1.5 / SDXL conv shapes, LoRA ranks 16-256, LoHa 16 / 32; DESIGN.md section 9), with E = N K / 1e6:
+        kernel     6 + 2.6 E + 0.11 L R       R = rank sums per element (LoRA r, LoHa r1 + r2), L = max(1, 64 x 128 tiles / 132 SMs)
+        two-step   per LoRA entry 8 + 9 E + 0.041 E r, per LoHa entry 16 + 15.4 E + 0.041 E (r1 + r2)
+    The kernel's rank loop costs more per rank than cuBLAS's product, so high ranks on small weights keep the two-step route
+    (LoRA above about rank 40 on a 320-channel 1x1 conv, about 120 on the SDXL 1280-channel 3x3)."""
+    E = N * K / 1e6
+    L = max(1.0, -(-N // 64) * -(-K // 128) / 132)
+    kernel, two_step = 6 + 2.6 * E, 0.0
+    for kind, _scale, factors, _sources in terms:
+        R = factors[0].shape[1] + (factors[2].shape[1] if kind == "loha" else 0)
+        kernel += 0.11 * L * R
+        two_step += (16 + 15.4 * E if kind == "loha" else 8 + 9 * E) + 0.041 * E * R
+    return kernel <= two_step
+
+
+def conv_patch_operands(terms, device):
+    """The fp32 factors of recognised `conv_patch_terms` on `device` and their ggufb200_lowrank_patch array (the tensors stay
+    referenced by the returned list for as long as the array is used)."""
+    ops = [(kind, scale, tuple(t.to(device=device, dtype=torch.float32).contiguous() for t in factors))
+           for kind, scale, factors, _sources in terms]
+
+    def desc(kind, scale, f):
+        loha = kind == "loha"
+        return _lib.LowrankPatch(f[0].data_ptr(), f[1].data_ptr(), f[2].data_ptr() if loha else None, f[3].data_ptr() if loha else None,
+                                 f[0].shape[1], f[2].shape[1] if loha else 0, scale)
+    return ops, (_lib.LowrankPatch * max(1, len(ops)))(*[desc(*op) for op in ops])
 
 
 def lokr_factor_shapes(factors):
@@ -1024,9 +1093,58 @@ class GGMLOps(comfy_ops.manual_cast):
             return torch.nn.functional.linear(input, weight, bias)
 
     class Conv2d(GGMLLayer, comfy_ops.manual_cast.Conv2d):
+        # LoRA / LoCon and LoHa patches (`conv_patch_terms`) on a packed weight: the patched weight [Cout, Cin, kh, kw] in one
+        # launch of ggufb200_dequant_lowrank, which forms each element's rank sums from staged factor tiles instead of
+        # dequantise + calculate_weight's fp32 [Cout, Cin kh kw] delta, scale, cast and add.  Same per-element rounding sequence;
+        # only the order of the rank sums differs from torch.mm.  Taken where its cost model says it wins (`lowrank_pays`: high
+        # ranks on small weights keep the two-step route).  False -> the reference's two-step arithmetic everywhere.
+        conv_patches_in_kernel = True
+
+        def _conv_patch_operands(self, input):
+            """`conv_patch_operands` of the weight's patch list, cached per patch set and device; None -> two-step route."""
+            w = self.weight
+            if not (self.conv_patches_in_kernel and input.is_cuda and input.dtype in _LOWRANK_ACT and is_quantized(w)
+                    and self.patch_dtype is None and not is_quantized(self.bias) and getattr(w, "patches", None)):
+                return None
+            qtype, shape = w.tensor_type, tuple(getattr(w, "tensor_shape", ()))
+            if qtype not in _LOWRANK_QTYPES or len(shape) != 4:
+                return None
+            N, K = shape[0], shape[1] * shape[2] * shape[3]
+            if K % 32 != 0 or (N * K) % gguf.GGML_QUANT_SIZES[qtype][0] != 0:
+                return None
+            terms = conv_patch_terms(_patch_entries(w))
+            if not terms or len(terms) > _lib.LOWRANK_MAX_PATCHES or not all(
+                    _fits_weight(kind, factors, None, N, K) and max(f.shape[0] for f in factors[1::2]) <= _lib.LOWRANK_MAX_RANK
+                    for kind, _s, factors, _src in terms) or not lowrank_pays(N, K, terms):
+                return None
+            dev = input.device
+            key = tuple((kind, float(scale)) + tuple(map(_tensor_key, sources)) for kind, scale, _f, sources in terms) + (str(dev),)
+            return _cached(self, "_gg_conv", key, lambda: conv_patch_operands(terms, dev))
+
         def forward_ggml_cast_weights(self, input):
-            weight, bias = self.cast_bias_weight(input)
-            return self._conv_forward(input, weight, bias)
+            operands = self._conv_patch_operands(input)
+            if operands is None:
+                weight, bias = self.cast_bias_weight(input)
+                return self._conv_forward(input, weight, bias)
+            dev, dtype = input.device, input.dtype
+            bias = None
+            if self.bias is not None:                                  # as cast_bias_weight brings it in, before the weight
+                async_ok = comfy_mm.device_supports_non_blocking(dev)
+                bias = comfy_ops.cast_to(self.get_weight(self.bias.to(dev), dtype), dtype, dev, non_blocking=async_ok, copy=False)
+            w = self.weight
+            qtype, shape = w.tensor_type, tuple(w.tensor_shape)
+            src = w.as_subclass(torch.Tensor)
+            wraw = src if src.device == dev else src.to(dev)           # offloaded module: packed bytes H2D for this call
+            if not wraw.is_contiguous():
+                wraw = wraw.contiguous()
+            ops, descs = operands
+            W = torch.empty(shape, dtype=dtype, device=dev)
+            N, K = shape[0], W.numel() // shape[0]
+            with torch.cuda.device(dev):
+                rc = _lib.lib().ggufb200_dequant_lowrank(int(qtype), wraw.data_ptr(), N, K, W.data_ptr(), dtype_code(dtype),
+                                                         math_code(self.dequant_dtype, dtype), descs, len(ops), _current_stream_ptr(dev.index))
+            _lib.check(rc, f"ggufb200_dequant_lowrank({getattr(qtype, 'name', qtype)}, N={N}, K={K})")
+            return self._conv_forward(input, W, bias)
 
     class Embedding(GGMLLayer, comfy_ops.manual_cast.Embedding):
         def forward_ggml_cast_weights(self, input, out_dtype=None):

@@ -170,6 +170,38 @@ int ggufb200_dequant_kron(int ggml_type, const void *packed, int64_t N, int64_t 
                           const ggufb200_kron_patch *patches, int n_patches, void *stream);
 
 /*
+ * Standalone dequant of an [N, K] weight with LoRA / LoCon and LoHa patches applied, in one launch.  Replaces, for a patched
+ * Conv2d (N = Cout, K = Cin * kh * kw), the reference's dequantise + comfy.lora.calculate_weight without its fp32 [N, K] delta.
+ * Every element of `out` is, patch by patch in list order,
+ *     W'[n, k] = out( W[n, k] + out( fp32(scale) * d[n, k] ) )
+ *     LoRA  d = sum_j a1[n, j] * b1[j, k]                                   (fp32, j ascending, one fused multiply-add per term)
+ *     LoHa  d = fp32( (sum_j a1[n, j] * b1[j, k]) * (sum_j a2[n, j] * b2[j, k]) )
+ * with out() = rounding to out_dtype and the sum W + delta formed in fp32: `weight += ((strength * alpha) * diff).type(dtype)` of
+ * ComfyUI's LoRA / LoHa adapters; only the order of the rank sums differs from the reference's torch.mm.  W is the
+ * ggufb200_dequant value in math_dtype cast to out_dtype; for the types of ggufb200_dequant_fallback it is that function's value
+ * (fp32, math_dtype is checked but not used).  math_dtype may carry GGUFB200_DEQUANT_SRC_STABLE (accepted, no effect).
+ *   packed     the flat block stream of the [N, K] matrix, any alignment: element n * K + k of the stream is W[n, k], so a
+ *              straddled weight (K % 256 != 0 with 256-element blocks) needs nothing special; K % 32 == 0, N * K a multiple of the
+ *              block size; not BF16 (GGUFB200_E_UNSUPPORTED)
+ *   out        N*K elements of out_dtype, 16-byte aligned
+ *   patches    host array of n_patches (0 .. GGUFB200_LOWRANK_MAX_PATCHES) descriptors; a1 / b1 / a2 / b2 are DEVICE pointers to
+ *              row-major fp32 matrices, 4-byte aligned (GGUFB200_E_ALIGN); a2 = NULL: LoRA (r2, b2 ignored), else LoHa.
+ *              1 <= r1, r2 <= GGUFB200_LOWRANK_MAX_RANK (GGUFB200_E_SHAPE)
+ */
+#define GGUFB200_LOWRANK_MAX_PATCHES 8
+#define GGUFB200_LOWRANK_MAX_RANK 1024
+typedef struct ggufb200_lowrank_patch {
+    const float *a1;       /* [N, r1]: LoRA up / LoHa w1a */
+    const float *b1;       /* [r1, K]: LoRA down / LoHa w1b */
+    const float *a2;       /* [N, r2]: LoHa w2a, NULL for LoRA */
+    const float *b2;       /* [r2, K]: LoHa w2b */
+    int64_t r1, r2;
+    float scale;           /* strength * alpha */
+} ggufb200_lowrank_patch;
+int ggufb200_dequant_lowrank(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
+                             const ggufb200_lowrank_patch *patches, int n_patches, void *stream);
+
+/*
  * Integer unpack only (test/debug surface for the "bit-exact integer unpack" contract):
  * per element the integer quant value q as it enters the float multiply, the integer
  * sub-block scale sc (1 if the type has none) and min mn (0 if none).  Any of the three
