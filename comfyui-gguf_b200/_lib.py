@@ -22,6 +22,7 @@ FLAG_W_STABLE = 0x4000          # ggufb200_linear: no kernel still in flight wri
 DEQUANT_SRC_STABLE = 0x100      # same promise for ggufb200_dequant, OR-ed into math_dtype
 OP_DEQUANT, OP_LINEAR, OP_ROWS, OP_LINEAR_MMA, OP_DEQUANT_FALLBACK = 0, 1, 2, 3, 4
 LOWRANK_MAX_PATCHES, LOWRANK_MAX_RANK = 8, 1024   # ggufb200_dequant_lowrank: descriptors per call, rank of one factor pair
+PATCH_LOWRANK, PATCH_KRON = 0, 1                   # ggufb200_weight_patch.kind
 
 
 class GGUFB200Error(RuntimeError):
@@ -39,6 +40,11 @@ class LowrankPatch(ctypes.Structure):
     """ggufb200_lowrank_patch (include/ggufb200.h): one LoRA (a2 = None) or LoHa patch of ggufb200_dequant_lowrank."""
     _fields_ = [("a1", ctypes.c_void_p), ("b1", ctypes.c_void_p), ("a2", ctypes.c_void_p), ("b2", ctypes.c_void_p), ("r1", ctypes.c_int64),
                 ("r2", ctypes.c_int64), ("scale", ctypes.c_float)]
+
+
+class WeightPatch(ctypes.Structure):
+    """ggufb200_weight_patch (include/ggufb200.h): one patch of ggufb200_dequant_patched, `lowrank` or `kron` as `kind` says."""
+    _fields_ = [("kind", ctypes.c_int32), ("lowrank", LowrankPatch), ("kron", KronPatch)]
 
 
 def build(verbose: bool = False) -> str:
@@ -72,6 +78,7 @@ def lib() -> ctypes.CDLL:
     L.ggufb200_dequant_fallback.argtypes = [c_int, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
     L.ggufb200_dequant_kron.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(KronPatch), c_int, c_vp]
     L.ggufb200_dequant_lowrank.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(LowrankPatch), c_int, c_vp]
+    L.ggufb200_dequant_patched.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(WeightPatch), c_int, c_vp]
     L.ggufb200_unpack_int.argtypes = [c_int, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]
     L.ggufb200_dequant_rows.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
     L.ggufb200_linear_plan.restype = c_int
@@ -112,5 +119,5 @@ EXPORTS = (
     "ggufb200_set_tuning", "ggufb200_linear_plan", "ggufb200_linear_workspace_ex",
     "ggufb200_repack_bytes", "ggufb200_repack", "ggufb200_linear_spans", "ggufb200_linear_lora",
     "ggufb200_linear_lora_ex", "ggufb200_dequant_kron", "ggufb200_dequant_fallback", "ggufb200_linear_lora_scaled",
-    "ggufb200_gemm_scaled", "ggufb200_scale_columns", "ggufb200_dequant_lowrank",
+    "ggufb200_gemm_scaled", "ggufb200_scale_columns", "ggufb200_dequant_lowrank", "ggufb200_dequant_patched",
 )

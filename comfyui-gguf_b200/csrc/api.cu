@@ -266,6 +266,55 @@ int ggufb200_dequant_lowrank(int ggml_type, const void *packed, int64_t N, int64
     return dequant_lowrank_dispatch(ggml_type, packed, N, K, out, out_dtype, math_dtype, patches, n_patches, (cudaStream_t)stream);
 }
 
+// a LOWRANK descriptor as ggufb200_dequant_lowrank checks it (0: fine)
+static int lowrank_patch_check(const ggufb200_lowrank_patch &p)
+{
+    const bool loha = p.a2 != nullptr;
+    if (p.r1 < 1 || p.r1 > GGUFB200_LOWRANK_MAX_RANK || (loha && (p.r2 < 1 || p.r2 > GGUFB200_LOWRANK_MAX_RANK))) return GGUFB200_E_SHAPE;
+    if (!p.a1 || !p.b1 || (loha && !p.b2)) return GGUFB200_E_NULL;
+    for (const float *f : {p.a1, p.b1, loha ? p.a2 : nullptr, loha ? p.b2 : nullptr})      // LoRA: b2 is not read
+        if (reinterpret_cast<uintptr_t>(f) & 3) return GGUFB200_E_ALIGN;
+    return GGUFB200_OK;
+}
+
+int ggufb200_dequant_patched(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
+                             const ggufb200_weight_patch *patches, int n_patches, void *stream)
+{
+    int bs = 0;
+    const bool fallback = with_fallback_block(ggml_type, false, [&](auto blk) {
+        bs = decltype(blk)::BS;
+        return true;
+    });
+    if (!fallback && !type_geom(ggml_type, &bs, nullptr)) return GGUFB200_E_TYPE;
+    if (ggml_type == T_BF16) return GGUFB200_E_UNSUPPORTED;
+    math_dtype &= ~GGUFB200_DEQUANT_SRC_STABLE;
+    if (!dtype_ok(out_dtype) || !dtype_ok(math_dtype)) return GGUFB200_E_DTYPE;
+    // grid: ceil(K / 128) x ceil(N / 64) CTAs, as ggufb200_dequant_lowrank
+    if (N <= 0 || K <= 0 || K % 32 != 0 || (N * K) % bs != 0 || N > 64ll * 65535 || K > 0x7fffffffll) return GGUFB200_E_SHAPE;
+    if (n_patches < 0 || n_patches > kLowrankMaxPatches) return GGUFB200_E_SHAPE;
+    if (n_patches > 0 && !patches) return GGUFB200_E_NULL;
+    for (int i = 0; i < n_patches; ++i) {
+        const ggufb200_weight_patch &p = patches[i];
+        if (p.kind == GGUFB200_PATCH_LOWRANK) {
+            if (int rc = lowrank_patch_check(p.lowrank)) return rc;
+        } else if (p.kind == GGUFB200_PATCH_KRON) {
+            const ggufb200_kron_patch &k = p.kron;
+            if (k.band_dim != -1) return GGUFB200_E_UNSUPPORTED;
+            if (k.a1 <= 0 || k.a2 <= 0 || k.b1 <= 0 || k.b2 <= 0 || k.a1 > N || k.b1 > N || k.a2 > K || k.b2 > K || k.a1 * k.b1 != N ||
+                k.a2 * k.b2 != K)
+                return GGUFB200_E_SHAPE;
+            if (!k.A || !k.B) return GGUFB200_E_NULL;
+            if ((reinterpret_cast<uintptr_t>(k.A) & 3) || (reinterpret_cast<uintptr_t>(k.B) & 3)) return GGUFB200_E_ALIGN;
+        } else {
+            return GGUFB200_E_UNSUPPORTED;
+        }
+    }
+    if (!packed || !out) return GGUFB200_E_NULL;
+    if (!aligned16(out)) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    return dequant_patched_dispatch(ggml_type, packed, N, K, out, out_dtype, math_dtype, patches, n_patches, (cudaStream_t)stream);
+}
+
 int ggufb200_unpack_int(int ggml_type,const void *packed, int64_t n_blocks, int16_t *q, int16_t *sc, int16_t *mn, void *stream)
 {
     if (!type_geom(ggml_type, nullptr, nullptr) || ggml_type == T_BF16) return GGUFB200_E_TYPE;

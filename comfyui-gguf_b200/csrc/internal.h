@@ -31,6 +31,9 @@ int dequant_kron_dispatch(int type, const void *packed, long long N, long long K
 constexpr int kLowrankMaxPatches = GGUFB200_LOWRANK_MAX_PATCHES;
 int dequant_lowrank_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
                              const ggufb200_lowrank_patch *patches, int n_patches, cudaStream_t st);
+// lowrank.cu, ggufb200_dequant_patched: the same with Kronecker (LoKr) patches as well; `patches` validated by the caller (api.cu)
+int dequant_patched_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
+                             const ggufb200_weight_patch *patches, int n_patches, cudaStream_t st);
 
 // ------------------------------------------------------------------ small-M Linear: gemv.cu (GGUFB200_ALGO_GEMV), gemv2.cu (GEMV_FAST)
 int gemv_max_m();

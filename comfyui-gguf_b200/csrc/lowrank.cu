@@ -14,6 +14,11 @@
 //   * w = out(w + out(fp32(scale) * d)) in list order, with d the rank sum (LoRA) or fp32(m1 * m2) of two (LoHa);
 //   * the tile leaves by 16-byte stores.
 // A kernel of its own: the K1 / kron / rows instances are untouched.
+//
+// ggufb200_dequant_patched runs the same tile with a third patch kind, Kronecker (LoKr), interleaved with LoRA / LoHa in list
+// order: d = fp32(A[n / b1, k / b2] * B[n % b1, k % b2]), A and B read through the read-only cache (one product per element, no
+// rank loop, nothing staged).  It is a kernel of its own (dequant_patched_kernel, the body shared as a compile-time variant), so
+// the dequant_lowrank_kernel instances compile exactly as without it.
 #include <type_traits>
 
 #include "blocks.cuh"
@@ -42,6 +47,18 @@ struct LowrankArgs {
     LowrankOp op[kLowrankMaxPatches];
     int n;
 };
+// ggufb200_dequant_patched: a LowrankOp, or (kron != 0) a Kronecker patch with A = lr.a1 [N / b1, a2], B = lr.b1 [b1, b2] and
+// lr.scale (N = a1 b1, K = a2 b2: the whole weight)
+struct PatchedOp {
+    LowrankOp lr;
+    int kron, a2, b1, b2;
+};
+struct PatchedArgs {
+    PatchedOp op[kLowrankMaxPatches];
+    int n;
+};
+__device__ __forceinline__ const LowrankOp &lowrank_of(const LowrankOp &op) { return op; }
+__device__ __forceinline__ const LowrankOp &lowrank_of(const PatchedOp &op) { return op.lr; }
 
 // shared-memory geometry of one (format, output dtype)
 template <class Q, int OUT> struct LrGeometry {
@@ -160,10 +177,52 @@ __device__ __forceinline__ void rank_sums(const float *__restrict__ a, const flo
     }
 }
 
-template <class Q, int MATH, int OUT>
-__global__ void __launch_bounds__(kThreads) dequant_lowrank_kernel(const uint8_t *__restrict__ src, long long total_bytes, int aligned, int N,
-                                                                   int K, uint8_t *__restrict__ dst, const __grid_constant__ LowrankArgs la)
+// The Kronecker patch on this thread's 4 x 8 block (rows n0 + 4 rg .., columns k0 + 8 cg ..; rows past N are skipped, the
+// caller skips a block past the tile's columns): w = out(w + out(fp32(scale) * fp32(A[i1, i2] * B[j1, j2]))), (i1, j1) =
+// divmod(n, b1), (i2, j2) = divmod(k, b2).
+template <int OUT, int PITCH>
+__device__ __forceinline__ void kron_block(uint8_t *otile, const PatchedOp &op, int N, int n0, int k0, int rg, int cg)
 {
+    constexpr int OB = OutT<OUT>::bytes;
+    const float *__restrict__ A = op.lr.a1;
+    const float *__restrict__ B = op.lr.b1;
+    const int kb = k0 + 8 * cg;
+    const int i2_0 = kb / op.b2, j2_0 = kb - i2_0 * op.b2;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int n = n0 + 4 * rg + i;
+        if (n >= N) break;
+        const int i1 = n / op.b1, j1 = n - i1 * op.b1;
+        const float *arow = A + (size_t)i1 * op.a2;
+        const float *brow = B + (size_t)j1 * op.b2;
+        uint8_t *w = otile + (4 * rg + i) * PITCH + 8 * cg * OB;
+        int i2 = i2_0, j2 = j2_0;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            const float d = __fmul_rn(__ldg(arow + i2), __ldg(brow + j2));
+            const float delta = to_f32<OUT>(to_out<OUT>(__fmul_rn(op.lr.scale, d)));
+            if constexpr (OUT == kF32) {
+                float &x = reinterpret_cast<float *>(w)[c];
+                x = __fadd_rn(x, delta);
+            } else {
+                uint16_t &x = reinterpret_cast<uint16_t *>(w)[c];
+                x = (uint16_t)to_out<OUT>(__fadd_rn(to_f32<OUT>(x), delta));
+            }
+            if (++j2 == op.b2) {
+                j2 = 0;
+                ++i2;
+            }
+        }
+    }
+}
+
+// The tile of one CTA; Args = LowrankArgs (ggufb200_dequant_lowrank) or PatchedArgs (ggufb200_dequant_patched, Kronecker
+// patches as well).
+template <class Q, int MATH, int OUT, class Args>
+__device__ __forceinline__ void lowrank_tile(const uint8_t *__restrict__ src, long long total_bytes, int aligned, int N, int K,
+                                             uint8_t *__restrict__ dst, const Args &la)
+{
+    constexpr bool KRON = std::is_same<Args, PatchedArgs>::value;
     using G = LrGeometry<Q, OUT>;
     constexpr int OB = G::OB;
     extern __shared__ __align__(16) uint8_t smem[];
@@ -208,7 +267,14 @@ __global__ void __launch_bounds__(kThreads) dequant_lowrank_kernel(const uint8_t
     // 3. the patches, in list order, on each thread's 4 x 8 block (rows 4 rg .., columns 8 cg ..)
     const int rg = tid / (kCols / 8), cg = tid % (kCols / 8);
     for (int p = 0; p < la.n; ++p) {
-        const LowrankOp &op = la.op[p];
+        if constexpr (KRON) {
+            if (la.op[p].kron) {
+                __syncthreads();                                  // the unpack (or the previous patch) of other threads' elements is done
+                if (8 * cg < cols) kron_block<OUT, G::PITCH>(otile, la.op[p], N, n0, k0, rg, cg);
+                continue;
+            }
+        }
+        const LowrankOp &op = lowrank_of(la.op[p]);
         float d[4][8];
         rank_sums(op.a1, op.b1, op.r1, N, K, n0, k0, stage, tid, d);
         if (op.r2 > 0) {
@@ -256,10 +322,31 @@ __global__ void __launch_bounds__(kThreads) dequant_lowrank_kernel(const uint8_t
 }
 
 template <class Q, int MATH, int OUT>
-int launch_lowrank(const void *packed, long long N, long long K, void *out, const LowrankArgs &la, cudaStream_t st)
+__global__ void __launch_bounds__(kThreads) dequant_lowrank_kernel(const uint8_t *__restrict__ src, long long total_bytes, int aligned, int N,
+                                                                   int K, uint8_t *__restrict__ dst, const __grid_constant__ LowrankArgs la)
+{
+    lowrank_tile<Q, MATH, OUT>(src, total_bytes, aligned, N, K, dst, la);
+}
+
+template <class Q, int MATH, int OUT>
+__global__ void __launch_bounds__(kThreads) dequant_patched_kernel(const uint8_t *__restrict__ src, long long total_bytes, int aligned, int N,
+                                                                   int K, uint8_t *__restrict__ dst, const __grid_constant__ PatchedArgs la)
+{
+    lowrank_tile<Q, MATH, OUT>(src, total_bytes, aligned, N, K, dst, la);
+}
+
+template <class Args, class Q, int MATH, int OUT> struct KernelOf {
+    static constexpr auto value = dequant_lowrank_kernel<Q, MATH, OUT>;
+};
+template <class Q, int MATH, int OUT> struct KernelOf<PatchedArgs, Q, MATH, OUT> {
+    static constexpr auto value = dequant_patched_kernel<Q, MATH, OUT>;
+};
+
+template <class Q, int MATH, int OUT, class Args>
+int launch_lowrank(const void *packed, long long N, long long K, void *out, const Args &la, cudaStream_t st)
 {
     using G = LrGeometry<Q, OUT>;
-    auto kern = dequant_lowrank_kernel<Q, MATH, OUT>;
+    auto kern = KernelOf<Args, Q, MATH, OUT>::value;
     static unsigned char smem_set[64] = {};
     if (!ensure_dynamic_smem(kern, G::SMEM, smem_set)) return GGUFB200_E_CUDA;
     const dim3 grid((unsigned)((K + kCols - 1) / kCols), (unsigned)((N + kRows - 1) / kRows));
@@ -270,7 +357,7 @@ int launch_lowrank(const void *packed, long long N, long long K, void *out, cons
     return cudaGetLastError() == cudaSuccess ? GGUFB200_OK : GGUFB200_E_CUDA;
 }
 
-template <class Q, int MATH> int lowrank_out(const void *p, long long N, long long K, void *out, int od, const LowrankArgs &la, cudaStream_t st)
+template <class Q, int MATH, class Args> int lowrank_out(const void *p, long long N, long long K, void *out, int od, const Args &la, cudaStream_t st)
 {
     switch (od) {
     case kF16: return launch_lowrank<Q, MATH, kF16>(p, N, K, out, la, st);
@@ -280,17 +367,11 @@ template <class Q, int MATH> int lowrank_out(const void *p, long long N, long lo
     return GGUFB200_E_DTYPE;
 }
 
-}  // namespace
-
-int dequant_lowrank_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
-                             const ggufb200_lowrank_patch *patches, int n_patches, cudaStream_t st)
+// every block format with K1's math dtypes, every fallback format in fp32, fp16 / bf16 / fp32 output
+template <class Args>
+int lowrank_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype, const Args &la,
+                     cudaStream_t st)
 {
-    LowrankArgs la{};
-    la.n = n_patches;
-    for (int i = 0; i < n_patches; ++i) {
-        const ggufb200_lowrank_patch &p = patches[i];
-        la.op[i] = LowrankOp{p.a1, p.b1, p.a2, p.b2, (int)p.r1, p.a2 ? (int)p.r2 : 0, p.scale};
-    }
     const int fb = with_fallback_block(type, (int)GGUFB200_E_TYPE, [&](auto blk) {     // fp32 math: the reference ignores dequant_dtype there
         return lowrank_out<decltype(blk), kF32>(packed, N, K, out, out_dtype, la, st);
     });
@@ -304,6 +385,44 @@ int dequant_lowrank_dispatch(int type, const void *packed, long long N, long lon
         }
         return (int)GGUFB200_E_DTYPE;
     });
+}
+
+LowrankOp lowrank_op(const ggufb200_lowrank_patch &p)
+{
+    return LowrankOp{p.a1, p.b1, p.a2, p.b2, (int)p.r1, p.a2 ? (int)p.r2 : 0, p.scale};
+}
+
+}  // namespace
+
+int dequant_lowrank_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
+                             const ggufb200_lowrank_patch *patches, int n_patches, cudaStream_t st)
+{
+    LowrankArgs la{};
+    la.n = n_patches;
+    for (int i = 0; i < n_patches; ++i) la.op[i] = lowrank_op(patches[i]);
+    return lowrank_dispatch(type, packed, N, K, out, out_dtype, math_dtype, la, st);
+}
+
+int dequant_patched_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
+                             const ggufb200_weight_patch *patches, int n_patches, cudaStream_t st)
+{
+    PatchedArgs la{};
+    la.n = n_patches;
+    for (int i = 0; i < n_patches; ++i) {
+        const ggufb200_weight_patch &p = patches[i];
+        PatchedOp &op = la.op[i];
+        if (p.kind == GGUFB200_PATCH_KRON) {
+            const ggufb200_kron_patch &k = p.kron;
+            op.lr = LowrankOp{k.A, k.B, nullptr, nullptr, 0, 0, k.scale};
+            op.kron = 1;
+            op.a2 = (int)k.a2;
+            op.b1 = (int)k.b1;
+            op.b2 = (int)k.b2;
+        } else {
+            op.lr = lowrank_op(p.lowrank);
+        }
+    }
+    return lowrank_dispatch(type, packed, N, K, out, out_dtype, math_dtype, la, st);
 }
 
 }  // namespace ggufb200

@@ -160,6 +160,10 @@ KRON_MAX_PATCHES = 8   # LoKr patches one ggufb200_dequant_kron call applies (cs
 # weight types and activation dtypes ggufb200_dequant_lowrank serves (every block format and numpy-fallback type but BF16)
 _LOWRANK_QTYPES = tuple(q for q in SUPPORTED_QTYPES if q != _Q.BF16) + FALLBACK_QTYPES
 _LOWRANK_ACT = (torch.float16, torch.bfloat16, torch.float32)
+# `lowrank_pays` terms of the conv LyCORIS entries (microseconds, tools/bench_conv_lycoris.py): the kernel's Kronecker pass per
+# tile wave; the two-step route's kron + scale + cast + add per LoKr entry (fixed + per million weight elements); the Tucker
+# composition (LoCon mid's mm and transposed copy, LoHa's two einsums) the two-step route adds per Tucker entry
+KRON_KERNEL_US, KRON_TWO_STEP_US, TUCKER_TWO_STEP_US = 1.5, (8.0, 10.0), 6.0
 
 
 def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None, scale=None):
@@ -460,20 +464,30 @@ def conv_patch_terms(patches):
 
 
 def lowrank_pays(N, K, terms):
-    """True when ggufb200_dequant_lowrank is expected to form the patched [N, K] weight faster than the two-step route (K1 +
-    calculate_weight).  Cost model in microseconds, fitted to tools/bench_conv_patches.py on an NVIDIA H100 80GB HBM3 at 700 W
-    (Q4_K, fp16, SD1.5 / SDXL conv shapes, LoRA ranks 16-256, LoHa 16 / 32; DESIGN.md section 9), with E = N K / 1e6:
-        kernel     6 + 2.6 E + 0.11 L R       R = rank sums per element (LoRA r, LoHa r1 + r2), L = max(1, 64 x 128 tiles / 132 SMs)
-        two-step   per LoRA entry 8 + 9 E + 0.041 E r, per LoHa entry 16 + 15.4 E + 0.041 E (r1 + r2)
+    """True when ggufb200_dequant_lowrank (or ggufb200_dequant_patched) is expected to form the patched [N, K] weight faster than
+    the two-step route (K1 + calculate_weight).  Cost model in microseconds, fitted to tools/bench_conv_patches.py and
+    tools/bench_conv_lycoris.py on an NVIDIA H100 80GB HBM3 at 700 W (Q4_K, fp16, SD1.5 / SDXL conv shapes, LoRA ranks 16-256,
+    LoHa 16 / 32, LoKr factors 4-16; DESIGN.md section 9), with E = N K / 1e6:
+        kernel     6 + 2.6 E + 0.11 L R + KRON_KERNEL_US L per LoKr entry
+                   R = rank sums per element (LoRA r, LoHa r1 + r2), L = max(1, 64 x 128 tiles / 132 SMs)
+        two-step   per LoRA entry 8 + 9 E + 0.041 E r, per LoHa entry 16 + 15.4 E + 0.041 E (r1 + r2),
+                   per LoKr entry KRON_TWO_STEP_US[0] + KRON_TWO_STEP_US[1] E
     The kernel's rank loop costs more per rank than cuBLAS's product, so high ranks on small weights keep the two-step route
-    (LoRA above about rank 40 on a 320-channel 1x1 conv, about 120 on the SDXL 1280-channel 3x3)."""
+    (LoRA above about rank 40 on a 320-channel 1x1 conv, about 120 on the SDXL 1280-channel 3x3).  LoCon `mid` and Tucker LoHa
+    entries are priced as the LoRA / LoHa they become, plus TUCKER_TWO_STEP_US on the two-step side for the Tucker products."""
     E = N * K / 1e6
     L = max(1.0, -(-N // 64) * -(-K // 128) / 132)
     kernel, two_step = 6 + 2.6 * E, 0.0
     for kind, _scale, factors, _sources in terms:
-        R = factors[0].shape[1] + (factors[2].shape[1] if kind == "loha" else 0)
+        if kind == "lokr":
+            kernel += KRON_KERNEL_US * L
+            two_step += KRON_TWO_STEP_US[0] + KRON_TWO_STEP_US[1] * E
+            continue
+        R = sum(conv_term_ranks(kind, factors))
         kernel += 0.11 * L * R
-        two_step += (16 + 15.4 * E if kind == "loha" else 8 + 9 * E) + 0.041 * E * R
+        two_step += (16 + 15.4 * E if kind in ("loha", "loha_tucker") else 8 + 9 * E) + 0.041 * E * R
+        if kind in ("locon_mid", "loha_tucker"):
+            two_step += TUCKER_TWO_STEP_US
     return kernel <= two_step
 
 
@@ -488,6 +502,225 @@ def conv_patch_operands(terms, device):
         return _lib.LowrankPatch(f[0].data_ptr(), f[1].data_ptr(), f[2].data_ptr() if loha else None, f[3].data_ptr() if loha else None,
                                  f[0].shape[1], f[2].shape[1] if loha else 0, scale)
     return ops, (_lib.LowrankPatch * max(1, len(ops)))(*[desc(*op) for op in ops])
+
+
+def _conv_lycoris_entry(entry):
+    """One whole-weight Conv2d patch entry of a form only `conv_lycoris_terms` serves, as (kind, scale, factors, sources), or None:
+        "locon_mid"    LoCon with a Tucker `mid`: factors (up, down, mid), a = alpha / down.shape[0]
+        "loha_tucker"  LoHa with both `t1` and `t2`: factors (w1a, w1b, t1, w2a, w2b, t2), a = alpha / w1b.shape[0]
+        "lokr"         LoKr, w1 whole 2-D or decomposed, w2 whole 2-D / 4-D, decomposed or Tucker (`t2`): factors (w1, w2, w1_a,
+                       w1_b, w2_a, w2_b, t2) with t2 None unless w2 is Tucker-decomposed, a = alpha / dim as `_decode_patch`
+    with scale = strength_patch * a and sources the entry's own tensors (cache keys).  None for an offset, DoRA, reshape,
+    strength_model != 1, a hook, only one of t1 / t2, a 4-D w1, factors that do not chain, and every plain LoRA / LoHa entry."""
+    if len(entry) < 3 or entry[2] != 1.0 or (len(entry) > 3 and entry[3] is not None) or (len(entry) > 4 and entry[4] is not None):
+        return None
+    value = entry[1]
+    kind = _ADAPTER_KINDS.get(type(value).__name__)
+    if kind is not None and hasattr(value, "weights"):
+        payload = tuple(value.weights)
+    elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] in ("lora", "loha", "lokr"):
+        kind, payload = value[0], tuple(value[1])
+    else:
+        return None
+
+    def dims(t, *n):
+        return torch.is_tensor(t) and t.dim() in n
+
+    def column(t):                                     # [r, c] or [r, c, 1, 1]: flatten(start_dim=1) keeps it a column factor
+        return dims(t, 2) or (dims(t, 4) and tuple(t.shape[2:]) == (1, 1))
+    if kind == "lora":
+        if len(payload) < 4:
+            return None
+        up, down, alpha, mid, dora_scale, reshape = (payload + (None,) * 2)[:6]
+        if mid is None or dora_scale is not None or reshape is not None or not (column(up) and column(down) and dims(mid, 4)):
+            return None
+        r = down.shape[0]
+        if up.shape[1] != r or tuple(mid.shape[:2]) != (r, r):
+            return None
+        factors, dim = (up, down, mid), r
+    elif kind == "loha":
+        if len(payload) < 7:
+            return None
+        w1a, w1b, alpha, w2a, w2b, t1, t2, dora_scale = (payload + (None,))[:8]
+        if t1 is None or t2 is None or dora_scale is not None or not all(dims(t, 2) for t in (w1a, w1b, w2a, w2b)) \
+                or not (dims(t1, 4) and dims(t2, 4)):
+            return None
+        if t1.shape[0] != w1a.shape[0] or t1.shape[1] != w1b.shape[0] or t2.shape[0] != w2a.shape[0] or t2.shape[1] != w2b.shape[0] \
+                or w1a.shape[1] != w2a.shape[1] or w1b.shape[1] != w2b.shape[1] or t1.shape[2:] != t2.shape[2:]:
+            return None
+        factors, dim = (w1a, w1b, t1, w2a, w2b, t2), w1b.shape[0]
+    else:
+        if len(payload) < 7:
+            return None
+        w1, w2, alpha, w1_a, w1_b, w2_a, w2_b, t2, dora_scale = (payload + (None,) * 2)[:9]
+        if dora_scale is not None:
+            return None
+        dim = None
+        if w1 is not None:
+            if not dims(w1, 2):
+                return None
+        elif dims(w1_a, 2) and dims(w1_b, 2) and w1_a.shape[1] == w1_b.shape[0]:
+            dim = w1_b.shape[0]
+        else:
+            return None
+        if w2 is not None:
+            if not dims(w2, 2, 4):
+                return None
+            t2 = None                                  # the reference reads t2 only for a decomposed w2
+        elif not (dims(w2_a, 2) and dims(w2_b, 2)):
+            return None
+        elif t2 is None:
+            if w2_a.shape[1] != w2_b.shape[0]:
+                return None
+            dim = w2_b.shape[0]
+        elif dims(t2, 4) and t2.shape[0] == w2_a.shape[0] and t2.shape[1] == w2_b.shape[0]:
+            dim = w2_b.shape[0]
+        else:
+            return None
+        factors = (w1, w2, w1_a, w1_b, w2_a, w2_b, t2)
+    a = 1.0 if alpha is None or dim is None else float(alpha) / dim
+    sources = tuple(t for t in factors if t is not None)
+    return {"lora": "locon_mid", "loha": "loha_tucker", "lokr": "lokr"}[kind], float(entry[0]) * a, factors, sources
+
+
+def conv_lycoris_terms(patches):
+    """Recognise a Conv2d patch list of whole-weight entries of which at least one is LoKr, LoCon with `mid` or Tucker LoHa
+    (`_conv_lycoris_entry`), mixed in any order with plain LoRA / LoCon and LoHa entries (`conv_patch_terms`).  Returns
+    [(kind, scale, factors, sources), ...] in list order, or None when the list has none of these entries (`conv_patch_terms`
+    serves it) or any entry needs `calculate_weight`."""
+    terms, lycoris = [], False
+    for entry in patches:
+        term = _conv_lycoris_entry(entry)
+        if term is None:
+            plain = conv_patch_terms([entry])
+            if not plain:
+                return None
+            term = plain[0]
+        else:
+            lycoris = True
+        terms.append(term)
+    return terms if lycoris else None
+
+
+def conv_lokr_shapes(factors):
+    """(a1, a2), (b1, b2) of a "lokr" conv term: A = w1 or w1_a @ w1_b, B = w2 (or its product / Tucker einsum) as [b1, b2]."""
+    w1, w2, w1_a, w1_b, w2_a, w2_b, t2 = factors
+    a = tuple(w1.shape) if w1 is not None else (w1_a.shape[0], w1_b.shape[1])
+    if w2 is not None:
+        b = (w2.shape[0], w2.numel() // w2.shape[0])
+    elif t2 is None:
+        b = (w2_a.shape[0], w2_b.shape[1])
+    else:
+        b = (w2_a.shape[1], w2_b.shape[1] * t2.shape[2] * t2.shape[3])
+    return a, b
+
+
+def conv_term_shape(kind, factors):
+    """(rows, cols) of the [N, K] delta of a `conv_lycoris_terms` term."""
+    if kind == "lokr":
+        (a1, a2), (b1, b2) = conv_lokr_shapes(factors)
+        return a1 * b1, a2 * b2
+    if kind == "locon_mid":
+        up, down, mid = factors
+        return up.shape[0], down.shape[1] * mid.shape[2] * mid.shape[3]
+    if kind == "loha_tucker":
+        w1a, w1b, t1 = factors[:3]
+        return w1a.shape[1], w1b.shape[1] * t1.shape[2] * t1.shape[3]
+    return factors[0].shape[0], factors[-1].shape[1]
+
+
+def conv_term_ranks(kind, factors):
+    """The ranks of a `conv_lycoris_terms` term's factor pairs (one for LoRA, two for LoHa, none for LoKr)."""
+    if kind == "lokr":
+        return ()
+    if kind == "locon_mid":
+        return (factors[1].shape[0],)
+    if kind == "loha_tucker":
+        return factors[2].shape[0], factors[5].shape[0]
+    return tuple(f.shape[0] for f in factors[1::2])
+
+
+def _reference_kron_raises(w1, w2):
+    """True when comfy.lora's `torch.kron(w1, w2)` (w1 unsqueezed to 4-D for a 4-D w2) raises for factors of these shapes and
+    strides: torch.kron views its product, which fails for some non-contiguous factors (a Tucker w2 straight out of
+    torch.einsum), and ComfyUI then logs the error and skips the entry.  Checked on meta tensors: no data is touched."""
+    m1 = torch.empty_strided(w1.shape, w1.stride(), device=_META)
+    m2 = torch.empty_strided(w2.shape, w2.stride(), device=_META)
+    if m2.dim() == 4:
+        m1 = m1.unsqueeze(2).unsqueeze(2)
+    try:
+        torch.kron(m1, m2)
+    except RuntimeError:
+        return True
+    return False
+
+
+def conv_lokr_operands(factors, device):
+    """fp32 A [a1, a2] and B [b1, K / a2] of a "lokr" conv term on `device`, each formed by comfy.lora's own expressions: a
+    decomposed factor is torch.mm of its halves, a Tucker w2 torch.einsum('i j k l, j r, i p -> p r k l', t2, w2_b, w2_a).  B's
+    2-D view makes torch.kron(w1, w2).reshape(Cout, -1) the 2-D Kronecker product of A and B.  None when the reference's
+    torch.kron raises for these factors (`_reference_kron_raises`): the entry is then the two-step route's to skip."""
+    w1, w2, w1_a, w1_b, w2_a, w2_b, t2 = factors
+
+    def f32(t):
+        return t.to(device=device, dtype=torch.float32)
+    A = f32(w1) if w1 is not None else torch.mm(f32(w1_a), f32(w1_b))
+    if w2 is not None:
+        B = f32(w2)
+    elif t2 is None:
+        B = torch.mm(f32(w2_a), f32(w2_b))
+    else:
+        B = torch.einsum("i j k l, j r, i p -> p r k l", f32(t2), f32(w2_b), f32(w2_a))
+    if _reference_kron_raises(A, B):
+        return None
+    return A.contiguous(), B.reshape(B.shape[0], -1).contiguous()
+
+
+def locon_mid_down(down, mid, device):
+    """LoCon's Tucker-composed down [r, Cin kh kw] in fp32 on `device`, by comfy.lora's expression (mm of the transposed down and
+    mid, reshaped and transposed back), flattened as calculate_weight multiplies it."""
+    down, mid = down.to(device=device, dtype=torch.float32), mid.to(device=device, dtype=torch.float32)
+    final_shape = [down.shape[1], down.shape[0], mid.shape[2], mid.shape[3]]
+    down = torch.mm(down.transpose(0, 1).flatten(start_dim=1), mid.transpose(0, 1).flatten(start_dim=1)).reshape(final_shape).transpose(0, 1)
+    return down.flatten(start_dim=1).contiguous()
+
+
+def loha_tucker_half(wa, wb, t, device):
+    """One Tucker LoHa half einsum('i j k l, j r, i p -> p r k l', t, wb, wa) as a rank-r product a @ b in fp32 on `device`:
+    a = wa^T [Cout, r], b = einsum('i j k l, j r -> i r k l', t, wb).reshape(r, Cin kh kw)."""
+    wa, wb, t = (x.to(device=device, dtype=torch.float32) for x in (wa, wb, t))
+    b = torch.einsum("i j k l, j r -> i r k l", t, wb)
+    return wa.t().contiguous(), b.reshape(b.shape[0], -1).contiguous()
+
+
+def conv_lycoris_operands(terms, device):
+    """The fp32 operands of recognised `conv_lycoris_terms` on `device` and their ggufb200_weight_patch array (the tensors stay
+    referenced by the returned list for as long as the array is used): LoRA / LoHa factors as they are, LoCon `mid` as a LoRA
+    with `locon_mid_down`, Tucker LoHa as a LoHa of `loha_tucker_half` pairs, LoKr as a Kronecker patch (`conv_lokr_operands`).
+    None when a LoKr entry is one the reference skips."""
+    keep, descs = [], []
+    for kind, scale, factors, _sources in terms:
+        if kind == "lokr":
+            AB = conv_lokr_operands(factors, device)
+            if AB is None:
+                return None
+            A, B = AB
+            keep.append(AB)
+            kron = _lib.KronPatch(A.data_ptr(), B.data_ptr(), A.shape[0], A.shape[1], B.shape[0], B.shape[1], -1, scale, 0, 0)
+            descs.append(_lib.WeightPatch(_lib.PATCH_KRON, _lib.LowrankPatch(), kron))
+            continue
+        if kind == "locon_mid":
+            f = (factors[0].to(device=device, dtype=torch.float32).flatten(start_dim=1).contiguous(), locon_mid_down(*factors[1:], device))
+        elif kind == "loha_tucker":
+            f = loha_tucker_half(*factors[:3], device) + loha_tucker_half(*factors[3:], device)
+        else:
+            f = tuple(t.to(device=device, dtype=torch.float32).contiguous() for t in factors)
+        keep.append(f)
+        loha = len(f) == 4
+        lowrank = _lib.LowrankPatch(f[0].data_ptr(), f[1].data_ptr(), f[2].data_ptr() if loha else None, f[3].data_ptr() if loha else None,
+                                    f[0].shape[1], f[2].shape[1] if loha else 0, scale)
+        descs.append(_lib.WeightPatch(_lib.PATCH_LOWRANK, lowrank, _lib.KronPatch()))
+    return keep, (_lib.WeightPatch * max(1, len(descs)))(*descs)
 
 
 def lokr_factor_shapes(factors):
@@ -1097,11 +1330,15 @@ class GGMLOps(comfy_ops.manual_cast):
         # launch of ggufb200_dequant_lowrank, which forms each element's rank sums from staged factor tiles instead of
         # dequantise + calculate_weight's fp32 [Cout, Cin kh kw] delta, scale, cast and add.  Same per-element rounding sequence;
         # only the order of the rank sums differs from torch.mm.  Taken where its cost model says it wins (`lowrank_pays`: high
-        # ranks on small weights keep the two-step route).  False -> the reference's two-step arithmetic everywhere.
+        # ranks on small weights keep the two-step route).
+        # Lists with LoKr, LoCon `mid` or Tucker LoHa entries (`conv_lycoris_terms`) take ggufb200_dequant_patched the same way,
+        # LoKr as a Kronecker patch (bit-identical to the reference's), the Tucker factors composed once per patch set.  (K1 with
+        # the Kronecker patch, ggufb200_dequant_kron, measured slower for LoKr factors 4 and 8 and within 4 % at 16.)
+        # False -> the reference's two-step arithmetic everywhere.
         conv_patches_in_kernel = True
 
-        def _conv_patch_operands(self, input):
-            """`conv_patch_operands` of the weight's patch list, cached per patch set and device; None -> two-step route."""
+        def _conv_kernel_shape(self, input):
+            """(qtype, N, K) of a patched packed weight the patch kernels can serve for this input, or None."""
             w = self.weight
             if not (self.conv_patches_in_kernel and input.is_cuda and input.dtype in _LOWRANK_ACT and is_quantized(w)
                     and self.patch_dtype is None and not is_quantized(self.bias) and getattr(w, "patches", None)):
@@ -1112,7 +1349,15 @@ class GGMLOps(comfy_ops.manual_cast):
             N, K = shape[0], shape[1] * shape[2] * shape[3]
             if K % 32 != 0 or (N * K) % gguf.GGML_QUANT_SIZES[qtype][0] != 0:
                 return None
-            terms = conv_patch_terms(_patch_entries(w))
+            return qtype, N, K
+
+        def _conv_patch_operands(self, input):
+            """`conv_patch_operands` of the weight's patch list, cached per patch set and device; None -> not served."""
+            geometry = self._conv_kernel_shape(input)
+            if geometry is None:
+                return None
+            _qtype, N, K = geometry
+            terms = conv_patch_terms(_patch_entries(self.weight))
             if not terms or len(terms) > _lib.LOWRANK_MAX_PATCHES or not all(
                     _fits_weight(kind, factors, None, N, K) and max(f.shape[0] for f in factors[1::2]) <= _lib.LOWRANK_MAX_RANK
                     for kind, _s, factors, _src in terms) or not lowrank_pays(N, K, terms):
@@ -1121,11 +1366,31 @@ class GGMLOps(comfy_ops.manual_cast):
             key = tuple((kind, float(scale)) + tuple(map(_tensor_key, sources)) for kind, scale, _f, sources in terms) + (str(dev),)
             return _cached(self, "_gg_conv", key, lambda: conv_patch_operands(terms, dev))
 
+        def _conv_lycoris_operands(self, input):
+            """`conv_lycoris_operands` of a list with LoKr / LoCon mid / Tucker LoHa entries (`conv_lycoris_terms`), cached per
+            patch set and device, where `lowrank_pays` expects ggufb200_dequant_patched to win; None -> two-step route."""
+            geometry = self._conv_kernel_shape(input)
+            if geometry is None:
+                return None
+            _qtype, N, K = geometry
+            terms = conv_lycoris_terms(_patch_entries(self.weight))
+            if not terms or len(terms) > _lib.LOWRANK_MAX_PATCHES or not all(
+                    conv_term_shape(kind, factors) == (N, K) and max(conv_term_ranks(kind, factors), default=0) <= _lib.LOWRANK_MAX_RANK
+                    for kind, _s, factors, _src in terms) or not lowrank_pays(N, K, terms):
+                return None
+            dev = input.device
+            key = tuple((kind, float(scale)) + tuple(map(_tensor_key, sources)) for kind, scale, _f, sources in terms) + (str(dev),)
+            # None (a LoKr entry the reference skips) is cached too
+            return _cached(self, "_gg_conv_lycoris", key, lambda: conv_lycoris_operands(terms, dev))
+
         def forward_ggml_cast_weights(self, input):
-            operands = self._conv_patch_operands(input)
+            entry, operands = "ggufb200_dequant_lowrank", self._conv_patch_operands(input)
+            if operands is None:
+                entry, operands = "ggufb200_dequant_patched", self._conv_lycoris_operands(input)
             if operands is None:
                 weight, bias = self.cast_bias_weight(input)
                 return self._conv_forward(input, weight, bias)
+            keep, descs = operands
             dev, dtype = input.device, input.dtype
             bias = None
             if self.bias is not None:                                  # as cast_bias_weight brings it in, before the weight
@@ -1137,13 +1402,12 @@ class GGMLOps(comfy_ops.manual_cast):
             wraw = src if src.device == dev else src.to(dev)           # offloaded module: packed bytes H2D for this call
             if not wraw.is_contiguous():
                 wraw = wraw.contiguous()
-            ops, descs = operands
             W = torch.empty(shape, dtype=dtype, device=dev)
             N, K = shape[0], W.numel() // shape[0]
             with torch.cuda.device(dev):
-                rc = _lib.lib().ggufb200_dequant_lowrank(int(qtype), wraw.data_ptr(), N, K, W.data_ptr(), dtype_code(dtype),
-                                                         math_code(self.dequant_dtype, dtype), descs, len(ops), _current_stream_ptr(dev.index))
-            _lib.check(rc, f"ggufb200_dequant_lowrank({getattr(qtype, 'name', qtype)}, N={N}, K={K})")
+                rc = getattr(_lib.lib(), entry)(int(qtype), wraw.data_ptr(), N, K, W.data_ptr(), dtype_code(dtype),
+                                                math_code(self.dequant_dtype, dtype), descs, len(keep), _current_stream_ptr(dev.index))
+            _lib.check(rc, f"{entry}({getattr(qtype, 'name', qtype)}, N={N}, K={K})")
             return self._conv_forward(input, W, bias)
 
     class Embedding(GGMLLayer, comfy_ops.manual_cast.Embedding):

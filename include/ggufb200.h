@@ -202,6 +202,32 @@ int ggufb200_dequant_lowrank(int ggml_type, const void *packed, int64_t N, int64
                              const ggufb200_lowrank_patch *patches, int n_patches, void *stream);
 
 /*
+ * ggufb200_dequant_lowrank with a third patch kind: LoKr (LyCORIS Kronecker) on the whole weight, in any mix and order with LoRA /
+ * LoCon and LoHa.  Replaces, for a Conv2d with LoKr or Tucker-factored LyCORIS patches, the reference's dequantise +
+ * comfy.lora.calculate_weight.  Every element of `out` is, patch by patch in list order,
+ *     W'[n, k] = out( W[n, k] + out( fp32(scale) * d[n, k] ) )
+ *     GGUFB200_PATCH_LOWRANK  d as in ggufb200_dequant_lowrank (`.lowrank`; a2 = NULL: LoRA, else LoHa)
+ *     GGUFB200_PATCH_KRON     d = fp32( A[n / b1, k / b2] * B[n % b1, k % b2] )   (`.kron`: A [a1, a2], B [b1, b2])
+ * A Kronecker element is the reference's `torch.kron(w1, w2).reshape(weight.shape)` element for element (B = w2 reshaped to
+ * [b1, K / a2]), so a list of Kronecker patches only gives the reference's patched weight bit for bit.  packed, out, N, K,
+ * out_dtype and math_dtype as in ggufb200_dequant_lowrank; only the descriptor of a patch's kind is read.
+ *   patches    host array of n_patches (0 .. GGUFB200_LOWRANK_MAX_PATCHES) descriptors of any mix of kinds.  Checked per patch:
+ *              an unknown kind, or a kron band_dim other than -1 (whole weight only): GGUFB200_E_UNSUPPORTED; a LOWRANK rank out of
+ *              range, a non-positive a1 / a2 / b1 / b2, a1 * b1 != N or a2 * b2 != K: GGUFB200_E_SHAPE; a NULL factor:
+ *              GGUFB200_E_NULL; a factor that is not 4-byte aligned: GGUFB200_E_ALIGN.  A and B are DEVICE pointers to
+ *              row-major fp32 matrices.
+ */
+#define GGUFB200_PATCH_LOWRANK 0   /* .lowrank: LoRA / LoCon (a2 == NULL) or LoHa */
+#define GGUFB200_PATCH_KRON 1      /* .kron: LoKr on the whole weight (band_dim must be -1) */
+typedef struct ggufb200_weight_patch {
+    int32_t kind;
+    ggufb200_lowrank_patch lowrank;
+    ggufb200_kron_patch kron;
+} ggufb200_weight_patch;
+int ggufb200_dequant_patched(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
+                             const ggufb200_weight_patch *patches, int n_patches, void *stream);
+
+/*
  * Integer unpack only (test/debug surface for the "bit-exact integer unpack" contract):
  * per element the integer quant value q as it enters the float multiply, the integer
  * sub-block scale sc (1 if the type has none) and min mn (0 if none).  Any of the three
