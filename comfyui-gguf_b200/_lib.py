@@ -23,6 +23,7 @@ DEQUANT_SRC_STABLE = 0x100      # same promise for ggufb200_dequant, OR-ed into 
 OP_DEQUANT, OP_LINEAR, OP_ROWS, OP_LINEAR_MMA, OP_DEQUANT_FALLBACK = 0, 1, 2, 3, 4
 LOWRANK_MAX_PATCHES, LOWRANK_MAX_RANK = 8, 1024   # ggufb200_dequant_lowrank: descriptors per call, rank of one factor pair
 PATCH_LOWRANK, PATCH_KRON = 0, 1                   # ggufb200_weight_patch.kind
+DORA_AXIS_OUT, DORA_AXIS_IN = 0, 1                 # ggufb200_dora_patch.axis
 
 
 class GGUFB200Error(RuntimeError):
@@ -45,6 +46,11 @@ class LowrankPatch(ctypes.Structure):
 class WeightPatch(ctypes.Structure):
     """ggufb200_weight_patch (include/ggufb200.h): one patch of ggufb200_dequant_patched, `lowrank` or `kron` as `kind` says."""
     _fields_ = [("kind", ctypes.c_int32), ("lowrank", LowrankPatch), ("kron", KronPatch)]
+
+
+class DoraPatch(ctypes.Structure):
+    """ggufb200_dora_patch (include/ggufb200.h): the DoRA step of one patch of ggufb200_dequant_patched_dora (factor None: plain)."""
+    _fields_ = [("factor", ctypes.c_void_p), ("axis", ctypes.c_int32), ("group", ctypes.c_int32), ("strength", ctypes.c_float)]
 
 
 def build(verbose: bool = False) -> str:
@@ -79,6 +85,8 @@ def lib() -> ctypes.CDLL:
     L.ggufb200_dequant_kron.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(KronPatch), c_int, c_vp]
     L.ggufb200_dequant_lowrank.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(LowrankPatch), c_int, c_vp]
     L.ggufb200_dequant_patched.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(WeightPatch), c_int, c_vp]
+    L.ggufb200_dequant_patched_dora.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_int, c_int, ctypes.POINTER(WeightPatch),
+                                                ctypes.POINTER(DoraPatch), c_int, c_vp]
     L.ggufb200_unpack_int.argtypes = [c_int, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]
     L.ggufb200_dequant_rows.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
     L.ggufb200_linear_plan.restype = c_int
@@ -120,4 +128,5 @@ EXPORTS = (
     "ggufb200_repack_bytes", "ggufb200_repack", "ggufb200_linear_spans", "ggufb200_linear_lora",
     "ggufb200_linear_lora_ex", "ggufb200_dequant_kron", "ggufb200_dequant_fallback", "ggufb200_linear_lora_scaled",
     "ggufb200_gemm_scaled", "ggufb200_scale_columns", "ggufb200_dequant_lowrank", "ggufb200_dequant_patched",
+    "ggufb200_dequant_patched_dora",
 )

@@ -277,8 +277,9 @@ static int lowrank_patch_check(const ggufb200_lowrank_patch &p)
     return GGUFB200_OK;
 }
 
-int ggufb200_dequant_patched(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
-                             const ggufb200_weight_patch *patches, int n_patches, void *stream)
+// the arguments of ggufb200_dequant_patched as it checks them (0: fine; the device is not checked)
+static int patched_args_check(int ggml_type, const void *packed, int64_t N, int64_t K, const void *out, int out_dtype, int math_dtype,
+                              const ggufb200_weight_patch *patches, int n_patches)
 {
     int bs = 0;
     const bool fallback = with_fallback_block(ggml_type, false, [&](auto blk) {
@@ -311,8 +312,33 @@ int ggufb200_dequant_patched(int ggml_type, const void *packed, int64_t N, int64
     }
     if (!packed || !out) return GGUFB200_E_NULL;
     if (!aligned16(out)) return GGUFB200_E_ALIGN;
+    return GGUFB200_OK;
+}
+
+int ggufb200_dequant_patched(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
+                             const ggufb200_weight_patch *patches, int n_patches, void *stream)
+{
+    if (int rc = patched_args_check(ggml_type, packed, N, K, out, out_dtype, math_dtype, patches, n_patches)) return rc;
     if (int rc = device_check()) return rc;
-    return dequant_patched_dispatch(ggml_type, packed, N, K, out, out_dtype, math_dtype, patches, n_patches, (cudaStream_t)stream);
+    return dequant_patched_dispatch(ggml_type, packed, N, K, out, out_dtype, math_dtype & ~GGUFB200_DEQUANT_SRC_STABLE, patches, n_patches,
+                                    (cudaStream_t)stream);
+}
+
+int ggufb200_dequant_patched_dora(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
+                                  const ggufb200_weight_patch *patches, const ggufb200_dora_patch *dora, int n_patches, void *stream)
+{
+    if (int rc = patched_args_check(ggml_type, packed, N, K, out, out_dtype, math_dtype, patches, n_patches)) return rc;
+    if (n_patches > 0 && !dora) return GGUFB200_E_NULL;
+    for (int i = 0; i < n_patches; ++i) {
+        const ggufb200_dora_patch &d = dora[i];
+        if (!d.factor) continue;
+        if (d.axis != GGUFB200_DORA_AXIS_OUT && d.axis != GGUFB200_DORA_AXIS_IN) return GGUFB200_E_SHAPE;
+        if (d.axis == GGUFB200_DORA_AXIS_IN && (d.group < 1 || K % d.group != 0)) return GGUFB200_E_SHAPE;
+        if (reinterpret_cast<uintptr_t>(d.factor) & 3) return GGUFB200_E_ALIGN;
+    }
+    if (int rc = device_check()) return rc;
+    return dequant_patched_dora_dispatch(ggml_type, packed, N, K, out, out_dtype, math_dtype & ~GGUFB200_DEQUANT_SRC_STABLE, patches, dora,
+                                         n_patches, (cudaStream_t)stream);
 }
 
 int ggufb200_unpack_int(int ggml_type,const void *packed, int64_t n_blocks, int16_t *q, int16_t *sc, int16_t *mn, void *stream)

@@ -32,6 +32,10 @@ constexpr int kLowrankMaxPatches = GGUFB200_LOWRANK_MAX_PATCHES;
 int dequant_lowrank_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
                              const ggufb200_lowrank_patch *patches, int n_patches, cudaStream_t st);
 // lowrank.cu, ggufb200_dequant_patched: the same with Kronecker (LoKr) patches as well; `patches` validated by the caller (api.cu)
+// lowrank.cu, ggufb200_dequant_patched_dora: the same with a DoRA step per patch (`dora`: n_patches descriptors, validated by
+// the caller)
+int dequant_patched_dora_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
+                                  const ggufb200_weight_patch *patches, const ggufb200_dora_patch *dora, int n_patches, cudaStream_t st);
 int dequant_patched_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
                              const ggufb200_weight_patch *patches, int n_patches, cudaStream_t st);
 

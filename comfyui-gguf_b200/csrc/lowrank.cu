@@ -19,6 +19,12 @@
 // order: d = fp32(A[n / b1, k / b2] * B[n % b1, k % b2]), A and B read through the read-only cache (one product per element, no
 // rank loop, nothing staged).  It is a kernel of its own (dequant_patched_kernel, the body shared as a compile-time variant), so
 // the dequant_lowrank_kernel instances compile exactly as without it.
+//
+// ggufb200_dequant_patched_dora is a third variant (dequant_patched_dora_kernel): any patch of the list may carry a DoRA step
+// (ComfyUI's weight_decompose with its factor s, computed by the caller), applied per element after the patch's delta:
+//     wc = out(w + out(fp32(scale) * d));  wc = out(wc * s[i]);  w = wc (strength 1) or out(w + out(st * out(wc - w)))
+// with i = n (output axis) or k / group (input axis: one factor per Conv2d input channel, group = kh kw); s read through the
+// read-only cache.  The two other variants compile exactly as without it.
 #include <type_traits>
 
 #include "blocks.cuh"
@@ -55,6 +61,17 @@ struct PatchedOp {
 };
 struct PatchedArgs {
     PatchedOp op[kLowrankMaxPatches];
+    int n;
+};
+// ggufb200_dequant_patched_dora: the PatchedOp list plus one DoRA step per patch (s == nullptr: a plain patch)
+struct DoraOp {
+    const float *s;                       // [N] (axis 0) or [K / group] (axis 1)
+    int axis, group, blend;               // blend: strength != 1
+    float strength;
+};
+struct DoraArgs {
+    PatchedOp op[kLowrankMaxPatches];
+    DoraOp dora[kLowrankMaxPatches];
     int n;
 };
 __device__ __forceinline__ const LowrankOp &lowrank_of(const LowrankOp &op) { return op; }
@@ -216,13 +233,82 @@ __device__ __forceinline__ void kron_block(uint8_t *otile, const PatchedOp &op, 
     }
 }
 
-// The tile of one CTA; Args = LowrankArgs (ggufb200_dequant_lowrank) or PatchedArgs (ggufb200_dequant_patched, Kronecker
-// patches as well).
+// DoRA variant: d[i][c] = fp32(A[i1, i2] * B[j1, j2]) of the Kronecker patch for this thread's 4 x 8 block (rows past N are
+// left as they are: `dora_block` skips them)
+__device__ __forceinline__ void kron_deltas(const PatchedOp &op, int N, int n0, int k0, int rg, int cg, float (&d)[4][8])
+{
+    const int kb = k0 + 8 * cg;
+    const int i2_0 = kb / op.b2, j2_0 = kb - i2_0 * op.b2;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int n = n0 + 4 * rg + i;
+        if (n >= N) break;
+        const int i1 = n / op.b1, j1 = n - i1 * op.b1;
+        const float *arow = op.lr.a1 + (size_t)i1 * op.a2;
+        const float *brow = op.lr.b1 + (size_t)j1 * op.b2;
+        int i2 = i2_0, j2 = j2_0;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            d[i][c] = __fmul_rn(__ldg(arow + i2), __ldg(brow + j2));
+            if (++j2 == op.b2) {
+                j2 = 0;
+                ++i2;
+            }
+        }
+    }
+}
+
+// DoRA variant: one patch on this thread's 4 x 8 block (rows past N skipped; the caller skips a block past the tile's columns):
+// wc = out(w + out(fp32(scale) * d)), then, for a DoRA patch, wc = out(wc * s[i]) and w = wc or out(w + out(st * out(wc - w))).
+// Every step rounds to the output dtype, as the reference's tensors of that dtype do.
+template <int OUT, int PITCH>
+__device__ __forceinline__ void dora_block(uint8_t *otile, const float (&d)[4][8], float scale, const DoraOp &dr, int N, int n0, int k0,
+                                           int rg, int cg)
+{
+    constexpr int OB = OutT<OUT>::bytes;
+    const bool in_axis = dr.s != nullptr && dr.axis == 1;
+    const int kb = k0 + 8 * cg;
+    // input axis: g = the channel of column kb + c, gk = the column's place in it (one division per patch, not per element)
+    int g = in_axis ? kb / dr.group : 0, gk = in_axis ? kb - g * dr.group : 0;
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+        const float s_col = in_axis ? __ldg(dr.s + g) : 0.0f;
+        if (in_axis && ++gk == dr.group) {
+            gk = 0;
+            ++g;
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int n = n0 + 4 * rg + i;
+            if (n >= N) break;
+            uint8_t *w = otile + (4 * rg + i) * PITCH + 8 * cg * OB;
+            float x;
+            if constexpr (OUT == kF32) x = reinterpret_cast<const float *>(w)[c];
+            else x = to_f32<OUT>(reinterpret_cast<const uint16_t *>(w)[c]);
+            const float delta = to_f32<OUT>(to_out<OUT>(__fmul_rn(scale, d[i][c])));
+            float wc = to_f32<OUT>(to_out<OUT>(__fadd_rn(x, delta)));
+            if (dr.s != nullptr) {
+                const float s = in_axis ? s_col : __ldg(dr.s + n);
+                wc = to_f32<OUT>(to_out<OUT>(__fmul_rn(wc, s)));
+                if (dr.blend) {
+                    const float t = to_f32<OUT>(to_out<OUT>(__fmul_rn(dr.strength, to_f32<OUT>(to_out<OUT>(__fsub_rn(wc, x))))));
+                    wc = to_f32<OUT>(to_out<OUT>(__fadd_rn(x, t)));
+                }
+            }
+            if constexpr (OUT == kF32) reinterpret_cast<float *>(w)[c] = wc;
+            else reinterpret_cast<uint16_t *>(w)[c] = (uint16_t)to_out<OUT>(wc);
+        }
+    }
+}
+
+// The tile of one CTA; Args = LowrankArgs (ggufb200_dequant_lowrank), PatchedArgs (ggufb200_dequant_patched, Kronecker
+// patches as well) or DoraArgs (ggufb200_dequant_patched_dora, a DoRA step per patch as well).
 template <class Q, int MATH, int OUT, class Args>
 __device__ __forceinline__ void lowrank_tile(const uint8_t *__restrict__ src, long long total_bytes, int aligned, int N, int K,
                                              uint8_t *__restrict__ dst, const Args &la)
 {
     constexpr bool KRON = std::is_same<Args, PatchedArgs>::value;
+    constexpr bool DORA = std::is_same<Args, DoraArgs>::value;
     using G = LrGeometry<Q, OUT>;
     constexpr int OB = G::OB;
     extern __shared__ __align__(16) uint8_t smem[];
@@ -267,6 +353,26 @@ __device__ __forceinline__ void lowrank_tile(const uint8_t *__restrict__ src, lo
     // 3. the patches, in list order, on each thread's 4 x 8 block (rows 4 rg .., columns 8 cg ..)
     const int rg = tid / (kCols / 8), cg = tid % (kCols / 8);
     for (int p = 0; p < la.n; ++p) {
+        if constexpr (DORA) {
+            const PatchedOp &op = la.op[p];
+            float d[4][8];
+            if (op.kron) {
+                __syncthreads();                                  // the unpack (or the previous patch) of other threads' elements is done
+                if (8 * cg < cols) kron_deltas(op, N, n0, k0, rg, cg, d);
+            } else {
+                rank_sums(op.lr.a1, op.lr.b1, op.lr.r1, N, K, n0, k0, stage, tid, d);
+                if (op.lr.r2 > 0) {
+                    float d2[4][8];
+                    rank_sums(op.lr.a2, op.lr.b2, op.lr.r2, N, K, n0, k0, stage, tid, d2);
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+#pragma unroll
+                        for (int c = 0; c < 8; ++c) d[i][c] = __fmul_rn(d[i][c], d2[i][c]);
+                }
+            }
+            if (8 * cg < cols) dora_block<OUT, G::PITCH>(otile, d, op.lr.scale, la.dora[p], N, n0, k0, rg, cg);
+            continue;
+        }
         if constexpr (KRON) {
             if (la.op[p].kron) {
                 __syncthreads();                                  // the unpack (or the previous patch) of other threads' elements is done
@@ -335,11 +441,22 @@ __global__ void __launch_bounds__(kThreads) dequant_patched_kernel(const uint8_t
     lowrank_tile<Q, MATH, OUT>(src, total_bytes, aligned, N, K, dst, la);
 }
 
+template <class Q, int MATH, int OUT>
+__global__ void __launch_bounds__(kThreads) dequant_patched_dora_kernel(const uint8_t *__restrict__ src, long long total_bytes, int aligned,
+                                                                        int N, int K, uint8_t *__restrict__ dst,
+                                                                        const __grid_constant__ DoraArgs la)
+{
+    lowrank_tile<Q, MATH, OUT>(src, total_bytes, aligned, N, K, dst, la);
+}
+
 template <class Args, class Q, int MATH, int OUT> struct KernelOf {
     static constexpr auto value = dequant_lowrank_kernel<Q, MATH, OUT>;
 };
 template <class Q, int MATH, int OUT> struct KernelOf<PatchedArgs, Q, MATH, OUT> {
     static constexpr auto value = dequant_patched_kernel<Q, MATH, OUT>;
+};
+template <class Q, int MATH, int OUT> struct KernelOf<DoraArgs, Q, MATH, OUT> {
+    static constexpr auto value = dequant_patched_dora_kernel<Q, MATH, OUT>;
 };
 
 template <class Q, int MATH, int OUT, class Args>
@@ -392,6 +509,22 @@ LowrankOp lowrank_op(const ggufb200_lowrank_patch &p)
     return LowrankOp{p.a1, p.b1, p.a2, p.b2, (int)p.r1, p.a2 ? (int)p.r2 : 0, p.scale};
 }
 
+PatchedOp patched_op(const ggufb200_weight_patch &p)
+{
+    PatchedOp op{};
+    if (p.kind == GGUFB200_PATCH_KRON) {
+        const ggufb200_kron_patch &k = p.kron;
+        op.lr = LowrankOp{k.A, k.B, nullptr, nullptr, 0, 0, k.scale};
+        op.kron = 1;
+        op.a2 = (int)k.a2;
+        op.b1 = (int)k.b1;
+        op.b2 = (int)k.b2;
+    } else {
+        op.lr = lowrank_op(p.lowrank);
+    }
+    return op;
+}
+
 }  // namespace
 
 int dequant_lowrank_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
@@ -408,19 +541,19 @@ int dequant_patched_dispatch(int type, const void *packed, long long N, long lon
 {
     PatchedArgs la{};
     la.n = n_patches;
+    for (int i = 0; i < n_patches; ++i) la.op[i] = patched_op(patches[i]);
+    return lowrank_dispatch(type, packed, N, K, out, out_dtype, math_dtype, la, st);
+}
+
+int dequant_patched_dora_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
+                                  const ggufb200_weight_patch *patches, const ggufb200_dora_patch *dora, int n_patches, cudaStream_t st)
+{
+    DoraArgs la{};
+    la.n = n_patches;
     for (int i = 0; i < n_patches; ++i) {
-        const ggufb200_weight_patch &p = patches[i];
-        PatchedOp &op = la.op[i];
-        if (p.kind == GGUFB200_PATCH_KRON) {
-            const ggufb200_kron_patch &k = p.kron;
-            op.lr = LowrankOp{k.A, k.B, nullptr, nullptr, 0, 0, k.scale};
-            op.kron = 1;
-            op.a2 = (int)k.a2;
-            op.b1 = (int)k.b1;
-            op.b2 = (int)k.b2;
-        } else {
-            op.lr = lowrank_op(p.lowrank);
-        }
+        la.op[i] = patched_op(patches[i]);
+        const ggufb200_dora_patch &d = dora[i];
+        la.dora[i] = DoraOp{d.factor, (int)d.axis, d.axis == 1 ? (int)d.group : 1, d.strength != 1.0f, d.strength};
     }
     return lowrank_dispatch(type, packed, N, K, out, out_dtype, math_dtype, la, st);
 }

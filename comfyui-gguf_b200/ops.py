@@ -164,6 +164,9 @@ _LOWRANK_ACT = (torch.float16, torch.bfloat16, torch.float32)
 # tile wave; the two-step route's kron + scale + cast + add per LoKr entry (fixed + per million weight elements); the Tucker
 # composition (LoCon mid's mm and transposed copy, LoHa's two einsums) the two-step route adds per Tucker entry
 KRON_KERNEL_US, KRON_TWO_STEP_US, TUCKER_TWO_STEP_US = 1.5, (8.0, 10.0), 6.0
+# `conv_dora_pays`: what weight_decompose's passes add to the two-step route per DoRA entry, net of the kernel's DoRA step (fixed,
+# per million weight elements; microseconds, the lower envelope over both axes and strengths in tools/bench_conv_dora.py)
+DORA_TWO_STEP_US = (9.0, 3.9)
 
 
 def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None, scale=None):
@@ -475,6 +478,12 @@ def lowrank_pays(N, K, terms):
     The kernel's rank loop costs more per rank than cuBLAS's product, so high ranks on small weights keep the two-step route
     (LoRA above about rank 40 on a 320-channel 1x1 conv, about 120 on the SDXL 1280-channel 3x3).  LoCon `mid` and Tucker LoHa
     entries are priced as the LoRA / LoHa they become, plus TUCKER_TWO_STEP_US on the two-step side for the Tucker products."""
+    kernel, two_step = _lowrank_costs(N, K, terms)
+    return kernel <= two_step
+
+
+def _lowrank_costs(N, K, terms):
+    """(kernel, two-step) microseconds of `lowrank_pays`'s cost model."""
     E = N * K / 1e6
     L = max(1.0, -(-N // 64) * -(-K // 128) / 132)
     kernel, two_step = 6 + 2.6 * E, 0.0
@@ -488,6 +497,20 @@ def lowrank_pays(N, K, terms):
         two_step += (16 + 15.4 * E if kind in ("loha", "loha_tucker") else 8 + 9 * E) + 0.041 * E * R
         if kind in ("locon_mid", "loha_tucker"):
             two_step += TUCKER_TWO_STEP_US
+    return kernel, two_step
+
+
+def conv_dora_pays(N, K, terms):
+    """True when ggufb200_dequant_patched_dora is expected to form the patched [N, K] weight of recognised `conv_dora_terms`
+    faster than the two-step route: `lowrank_pays`'s model of the deltas, plus on the two-step side weight_decompose's passes
+    per DoRA entry (alpha scale, cast, add, norm, division, factor scale and, at strength != 1, the blend), net of the kernel's
+    DoRA step: DORA_TWO_STEP_US fixed + per million weight elements.  Measured on an NVIDIA H100 80GB HBM3 at 700 W (Q4_K / Q8_0,
+    fp16, SD1.5 / SDXL conv shapes, DoRA LoCon ranks 16-64, LoHa 16, LoKr factor 8; DESIGN.md section 9) the kernel won in every
+    row, including rank 64 on the 320-channel 1x1 conv, where the plain LoRA keeps the two-step route."""
+    kernel, two_step = _lowrank_costs(N, K, [(kind, st * a, factors, sources) for kind, st, a, factors, sources, _ds, _axis in terms])
+    for *_t, ds, _axis in terms:
+        if ds is not None:
+            two_step += DORA_TWO_STEP_US[0] + DORA_TWO_STEP_US[1] * N * K / 1e6
     return kernel <= two_step
 
 
@@ -723,6 +746,119 @@ def conv_lycoris_operands(terms, device):
     return keep, (_lib.WeightPatch * max(1, len(descs)))(*descs)
 
 
+_DORA_AT = {"lora": 4, "loha": 7, "lokr": 8}      # index of dora_scale in a LoRA / LoHa / LoKr payload
+
+
+def _split_dora(entry):
+    """(entry', dora_scale) of a LoRA / LoHa / LoKr patch entry: entry' is the entry at strength 1 with its value as a (kind,
+    payload) pair whose dora_scale is None, dora_scale the entry's own (None when it has none).  (None, None) for another value."""
+    value = entry[1] if len(entry) > 1 else None
+    kind = _ADAPTER_KINDS.get(type(value).__name__)
+    if kind is not None and hasattr(value, "weights"):
+        payload = tuple(value.weights)
+    elif isinstance(value, (tuple, list)) and len(value) == 2 and value[0] in _DORA_AT:
+        kind, payload = value[0], tuple(value[1])
+    else:
+        return None, None
+    at = _DORA_AT[kind]
+    dora_scale = payload[at] if len(payload) > at else None
+    if dora_scale is not None:
+        payload = payload[:at] + (None,) + payload[at + 1:]
+    return (1.0, (kind, payload)) + tuple(entry[2:]), dora_scale
+
+
+def conv_dora_axis(dora_scale, shape):
+    """weight_decompose's axis for a Conv2d weight of `shape` [Cout, Cin, kh, kw]: 0 for dora_scale [Cout, 1, 1, 1] (one norm per
+    output channel), 1 for [1, Cin, 1, 1] (one per input channel), None for any other shape.  The reference normalises the output
+    axis when dora_scale.shape[0] == Cout."""
+    cout, cin = shape[0], shape[1]
+    ds = tuple(dora_scale.shape)
+    if ds == (cout, 1, 1, 1):
+        return 0
+    if ds == (1, cin, 1, 1) and cout != 1:
+        return 1
+    return None
+
+
+def conv_dora_terms(patches, shape):
+    """Recognise a Conv2d patch list of whole-weight entries of which at least one carries DoRA (`dora_scale`), for a weight of
+    `shape` [Cout, Cin, kh, kw].  Every entry, its dora_scale set aside (`_split_dora`), is one `conv_patch_terms` or
+    `conv_lycoris_terms` serve: LoRA / LoCon (with or without `mid`), LoHa (plain or Tucker) and LoKr, in any order.  Returns
+    [(kind, strength, a, factors, sources, dora_scale, axis), ...] in list order (a = alpha / rank, kept apart from the strength;
+    sources the entry's tensors, dora_scale included, as cache keys; dora_scale and axis None for a plain entry), or None when
+    the list has no DoRA entry (the other recognisers serve it), has more than LOWRANK_MAX_PATCHES entries, or any entry needs
+    `calculate_weight` (strength_model != 1, a hook, an offset, reshape), does not fit [Cout, Cin kh kw], exceeds the rank limit,
+    has a dora_scale that is not a tensor of a `conv_dora_axis` shape, or a strength != 1 that rounds to 1 in fp32."""
+    if len(patches) > _lib.LOWRANK_MAX_PATCHES:
+        return None
+    N, K = shape[0], shape[1] * shape[2] * shape[3]
+    terms = []
+    for entry in patches:
+        unit, dora_scale = _split_dora(entry)
+        if unit is None:
+            return None
+        term = _conv_lycoris_entry(unit)
+        if term is None:
+            plain = conv_patch_terms([unit])
+            if not plain:
+                return None
+            term = plain[0]
+        kind, a, factors, sources = term
+        if conv_term_shape(kind, factors) != (N, K) or max(conv_term_ranks(kind, factors), default=0) > _lib.LOWRANK_MAX_RANK:
+            return None
+        strength, axis = float(entry[0]), None
+        if dora_scale is not None:
+            if not torch.is_tensor(dora_scale):
+                return None
+            axis = conv_dora_axis(dora_scale, shape)
+            if axis is None or (strength != 1.0 and float(torch.tensor(strength, dtype=torch.float32)) == 1.0):
+                return None
+            sources = tuple(sources) + (dora_scale,)
+        terms.append((kind, strength, a, factors, tuple(sources), dora_scale, axis))
+    return terms if any(t[5] is not None for t in terms) else None
+
+
+def conv_term_delta(kind, factors, device):
+    """The fp32 [N, K] delta of a `conv_dora_terms` term as ComfyUI's adapters form it (`calculate_weight`, before scaling):
+    LoRA torch.mm of the flattened factors (LoCon `mid`: of the composed down, `locon_mid_down`), LoHa the product of two torch.mm
+    (Tucker: of two einsum('i j k l, j r, i p -> p r k l', t, wb, wa)), LoKr the Kronecker product (`conv_lokr_operands`; None
+    when the reference skips the entry)."""
+    def f32(t):
+        return t.to(device=device, dtype=torch.float32)
+    if kind == "lokr":
+        AB = conv_lokr_operands(factors, device)
+        return None if AB is None else torch.kron(*AB)
+    if kind == "locon_mid":
+        return torch.mm(f32(factors[0]).flatten(start_dim=1), locon_mid_down(*factors[1:], device))
+    if kind == "loha_tucker":
+        w1a, w1b, t1, w2a, w2b, t2 = (f32(t) for t in factors)
+        m1 = torch.einsum("i j k l, j r, i p -> p r k l", t1, w1b, w1a)
+        m2 = torch.einsum("i j k l, j r, i p -> p r k l", t2, w2b, w2a)
+        return (m1 * m2).reshape(m1.shape[0], -1)
+    return _dora_delta(kind, factors, device)
+
+
+def build_conv_dora_plan(W, terms):
+    """The cached operands of ggufb200_dequant_patched_dora for recognised `conv_dora_terms` on the dequantised weight W
+    ([Cout, Cin, kh, kw] in the activation dtype, on the device of the forward): (tensors to keep, ggufb200_weight_patch array,
+    ggufb200_dora_patch array).  The factors s are the reference's own, `dora_replay` of the entries on W; the deltas' operands
+    are `conv_lycoris_operands`' with scale alpha for a DoRA entry (the kernel applies its strength in the DoRA step) and
+    strength * alpha for a plain one.  None when an entry is a LoKr entry the reference skips."""
+    if any(kind == "lokr" and conv_lokr_operands(f, W.device) is None for kind, _st, _a, f, *_rest in terms):
+        return None
+    factors, _patched = dora_replay(W, [(kind, st, a, f, ds) for kind, st, a, f, _src, ds, _axis in terms], conv_term_delta)
+    operands = conv_lycoris_operands([(kind, a if ds is not None else st * a, f, src) for kind, st, a, f, src, ds, _axis in terms], W.device)
+    if operands is None:
+        return None
+    keep, descs = operands
+    group = W.shape[2] * W.shape[3]
+    s32 = [None if s is None else s.float().contiguous() for s in factors]
+    dora = (_lib.DoraPatch * max(1, len(terms)))(*[
+        _lib.DoraPatch() if s is None else _lib.DoraPatch(s.data_ptr(), axis, group, st)
+        for (_kind, st, _a, _f, _src, _ds, axis), s in zip(terms, s32)])
+    return (keep, s32), descs, dora
+
+
 def lokr_factor_shapes(factors):
     """(a1, a2), (b1, b2) of a recognised LoKr term's A = w1 (or w1_a @ w1_b) and B = w2 (or w2_a @ w2_b)."""
     w1, w2, w1_a, w1_b, w2_a, w2_b = factors
@@ -874,21 +1010,24 @@ def _dora_delta(kind, factors, device):
     return torch.mm(f[0], f[1]) * torch.mm(f[2], f[3])
 
 
-def dora_replay(W, terms):
-    """The reference's calculate_weight over recognised `dora_terms` on W ([N, K] in the activation dtype, the dequantised weight;
-    not modified), in the same ops, dtype and device.  Returns each entry's DoRA factor s (W's dtype, [N] for the output axis,
-    [K] for the input axis; None for an entry without DoRA) and the patched weight.  Per entry with strength st and alpha a:
+def dora_replay(W, terms, delta_of=_dora_delta):
+    """The reference's calculate_weight over recognised `dora_terms` on W ([N, K] in the activation dtype, the dequantised weight,
+    or a Conv2d's [Cout, Cin, kh, kw]; not modified), in the same ops, dtype and device.  Returns each entry's DoRA factor s (W's
+    dtype, [N] / [Cout] for the output axis, [K] / [Cin] for the input axis; None for an entry without DoRA) and the patched
+    weight.  Per entry with strength st and alpha a, delta = delta_of(kind, factors, device) as calculate_weight forms it:
         plain   W += ((st * a) * delta).to(W.dtype)
         DoRA    Wc = W + (delta * a).to(W.dtype)
-                nrm = row norms of W (output axis: the weight BEFORE this patch) or column norms of Wc (input axis), + eps(W.dtype)
+                nrm = norms of W's rows W.reshape(N, -1) (output axis: the weight BEFORE this patch) or of Wc's input slices
+                      Wc.transpose(0, 1).reshape(W.shape[1], -1) (input axis), + eps(W.dtype)
                 s = (fp32(dora_scale) / nrm).to(W.dtype);  Wc *= s
                 W = Wc if st == 1 else W + st * (Wc - W)"""
     W = W.clone()
-    N, K = W.shape
+    N = W.shape[0]
+    ones = [1] * (W.dim() - 1)
     eps = torch.finfo(W.dtype).eps
     factors = []
     for kind, strength, alpha, fac, dora_scale in terms:
-        delta = _dora_delta(kind, fac, W.device)
+        delta = delta_of(kind, fac, W.device).reshape(W.shape)
         if dora_scale is None:
             W += ((strength * alpha) * delta).to(W.dtype)
             factors.append(None)
@@ -896,9 +1035,10 @@ def dora_replay(W, terms):
         delta *= alpha
         Wc = W + delta.to(W.dtype)
         if dora_scale.shape[0] == N:
-            nrm = W.reshape(N, -1).norm(dim=1, keepdim=True)
+            nrm = W.reshape(N, -1).norm(dim=1, keepdim=True).reshape(N, *ones)
         else:
-            nrm = Wc.transpose(0, 1).reshape(K, -1).norm(dim=1, keepdim=True).transpose(0, 1)
+            C = W.shape[1]
+            nrm = Wc.transpose(0, 1).reshape(C, -1).norm(dim=1, keepdim=True).reshape(C, *ones).transpose(0, 1)
         nrm = nrm + eps
         s = (dora_scale.to(device=W.device, dtype=torch.float32) / nrm).to(W.dtype)
         Wc *= s
@@ -1334,6 +1474,9 @@ class GGMLOps(comfy_ops.manual_cast):
         # Lists with LoKr, LoCon `mid` or Tucker LoHa entries (`conv_lycoris_terms`) take ggufb200_dequant_patched the same way,
         # LoKr as a Kronecker patch (bit-identical to the reference's), the Tucker factors composed once per patch set.  (K1 with
         # the Kronecker patch, ggufb200_dequant_kron, measured slower for LoKr factors 4 and 8 and within 4 % at 16.)
+        # Lists with DoRA entries (`conv_dora_terms`) take ggufb200_dequant_patched_dora: the factors s of weight_decompose are
+        # replayed once per patch set on the dequantised weight (`build_conv_dora_plan`), and the kernel applies each entry's
+        # delta, factor and strength blend per element, in the reference's rounding sequence.
         # False -> the reference's two-step arithmetic everywhere.
         conv_patches_in_kernel = True
 
@@ -1383,10 +1526,41 @@ class GGMLOps(comfy_ops.manual_cast):
             # None (a LoKr entry the reference skips) is cached too
             return _cached(self, "_gg_conv_lycoris", key, lambda: conv_lycoris_operands(terms, dev))
 
+        def _conv_dora_plan(self, input):
+            """`build_conv_dora_plan` of a list with DoRA entries (`conv_dora_terms`), cached per patch set and activation dtype
+            (one slot per dtype), where `conv_dora_pays` expects ggufb200_dequant_patched_dora to win; None -> two-step route.
+            The key holds every factor and dora_scale (identity, storage, version), the strengths, the packed weight (identity,
+            storage, version), the device and dequant_dtype: the factors s depend on all of them."""
+            geometry = self._conv_kernel_shape(input)
+            if geometry is None:
+                return None
+            _qtype, N, K = geometry
+            w = self.weight
+            shape = tuple(w.tensor_shape)
+            terms = conv_dora_terms(_patch_entries(w), shape)
+            if terms is None or not conv_dora_pays(N, K, terms):
+                return None
+            dev, dtype = input.device, input.dtype
+            src = w.as_subclass(torch.Tensor)
+            key = tuple((kind, st, a) + tuple(map(_tensor_key, sources)) for kind, st, a, _f, sources, _ds, _axis in terms) \
+                + (id(w), src.data_ptr(), src._version, str(dev), self.dequant_dtype)
+
+            def build():
+                W = _plain(dequantize_tensor(w if src.device == dev else w.to(dev), dtype, self.dequant_dtype))
+                return build_conv_dora_plan(W, terms)
+            # None (a LoKr entry the reference skips) is cached too
+            return _cached(self, "_gg_conv_dora_" + str(dtype).split(".")[-1], key, build)
+
         def forward_ggml_cast_weights(self, input):
             entry, operands = "ggufb200_dequant_lowrank", self._conv_patch_operands(input)
             if operands is None:
                 entry, operands = "ggufb200_dequant_patched", self._conv_lycoris_operands(input)
+            dora = None
+            if operands is None:
+                plan = self._conv_dora_plan(input)
+                if plan is not None:
+                    entry, (keep, _s), descs, dora = "ggufb200_dequant_patched_dora", *plan
+                    operands = keep, descs
             if operands is None:
                 weight, bias = self.cast_bias_weight(input)
                 return self._conv_forward(input, weight, bias)
@@ -1404,9 +1578,10 @@ class GGMLOps(comfy_ops.manual_cast):
                 wraw = wraw.contiguous()
             W = torch.empty(shape, dtype=dtype, device=dev)
             N, K = shape[0], W.numel() // shape[0]
+            args = (descs, len(keep)) if dora is None else (descs, dora, len(keep))
             with torch.cuda.device(dev):
                 rc = getattr(_lib.lib(), entry)(int(qtype), wraw.data_ptr(), N, K, W.data_ptr(), dtype_code(dtype),
-                                                math_code(self.dequant_dtype, dtype), descs, len(keep), _current_stream_ptr(dev.index))
+                                                math_code(self.dequant_dtype, dtype), *args, _current_stream_ptr(dev.index))
             _lib.check(rc, f"{entry}({getattr(qtype, 'name', qtype)}, N={N}, K={K})")
             return self._conv_forward(input, W, bias)
 

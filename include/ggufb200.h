@@ -228,6 +228,34 @@ int ggufb200_dequant_patched(int ggml_type, const void *packed, int64_t N, int64
                              const ggufb200_weight_patch *patches, int n_patches, void *stream);
 
 /*
+ * ggufb200_dequant_patched with DoRA (weight-decomposed LoRA) steps.  Replaces, for a Conv2d whose patch list carries
+ * `dora_scale` entries, the reference's dequantise + comfy.lora.calculate_weight with its weight_decompose.  `dora` is a host
+ * array parallel to `patches`; a descriptor with factor == NULL leaves its patch plain (as in ggufb200_dequant_patched).  For a
+ * patch with a factor, element by element in list order, with d the patch's delta (any kind) and out() = rounding to out_dtype:
+ *     wc = out( W[n, k] + out( fp32(scale) * d[n, k] ) )          scale = alpha, without the strength
+ *     wc = out( wc * factor[i] )                                   i = n (axis 0) or k / group (axis 1)
+ *     W'[n, k] = wc                                                strength == 1
+ *     W'[n, k] = out( W[n, k] + out( strength * out(wc - W[n, k]) ) )   otherwise
+ * which is weight_decompose's `Wc = W + (delta * alpha).to(dtype); Wc *= s; W = Wc` or `Wc -= W; W += strength * Wc` once its
+ * factor s = (dora_scale / (norm + eps)).to(dtype) is known: the caller forms s (it depends only on the weight and the patch
+ * set) and passes it as fp32 holding the dtype values.  The sums and products are formed in fp32.
+ *   dora       host array of n_patches descriptors (NULL: GGUFB200_E_NULL when n_patches > 0).  Per descriptor with a factor:
+ *              an axis other than 0 / 1, a group < 1 or K % group != 0 on axis 1: GGUFB200_E_SHAPE; a factor that is not 4-byte
+ *              aligned: GGUFB200_E_ALIGN.  factor is a DEVICE pointer to N (axis 0) or K / group (axis 1) fp32 values.
+ * Everything else as ggufb200_dequant_patched, checked the same way.
+ */
+#define GGUFB200_DORA_AXIS_OUT 0   /* one factor per output row (weight_decompose's output axis, LyCORIS wd_on_out) */
+#define GGUFB200_DORA_AXIS_IN 1    /* one factor per group of `group` input columns (a Conv2d input channel: group = kh * kw) */
+typedef struct ggufb200_dora_patch {
+    const float *factor;   /* NULL: a plain patch; else s, [N] or [K / group] */
+    int32_t axis;          /* GGUFB200_DORA_AXIS_OUT or GGUFB200_DORA_AXIS_IN */
+    int32_t group;         /* input columns per factor (axis 1); not read on axis 0 */
+    float strength;        /* strength_patch of the entry: 1 -> W' = wc */
+} ggufb200_dora_patch;
+int ggufb200_dequant_patched_dora(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
+                                  const ggufb200_weight_patch *patches, const ggufb200_dora_patch *dora, int n_patches, void *stream);
+
+/*
  * Integer unpack only (test/debug surface for the "bit-exact integer unpack" contract):
  * per element the integer quant value q as it enters the float multiply, the integer
  * sub-block scale sc (1 if the type has none) and min mn (0 if none).  Any of the three
