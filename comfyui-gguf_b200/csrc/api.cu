@@ -1,6 +1,6 @@
 // api.cu -- the extern "C" boundary declared in include/ggufb200.h.
 // Argument validation and route selection live here; kernels live in dequant.cu / rows.cu / gemv.cu / gemv2.cu /
-// linear_sm90.cu / repack.cu / scale.cu (declared in internal.h).  Routing is a pure function of the call's arguments (algo | flags):
+// linear_sm90.cu / repack.cu / scale.cu / lowrank.cu / quantize.cu (declared in internal.h).  Routing is a pure function of the call's arguments (algo | flags):
 // no process-wide routing state.
 #include <stdlib.h>
 
@@ -148,6 +148,7 @@ int ggufb200_type_info(int ggml_type, int *block_size, int *type_size)
 int ggufb200_supported(int ggml_type, int op)
 {
     if (op == GGUFB200_OP_DEQUANT_FALLBACK) return with_fallback_block(ggml_type, 0, [](auto) { return 1; });
+    if (op == GGUFB200_OP_QUANTIZE) return quantize_supported(ggml_type) ? 1 : 0;
     if (!type_geom(ggml_type, nullptr, nullptr)) return 0;
     switch (op) {
     case GGUFB200_OP_DEQUANT: return 1;
@@ -201,6 +202,19 @@ int ggufb200_dequant_fallback(int ggml_type, const void *packed, int64_t n_block
     if (!aligned16(out)) return GGUFB200_E_ALIGN;
     if (int rc = device_check()) return rc;
     return fallback_dispatch(ggml_type, packed, n_blocks, out, out_dtype, (cudaStream_t)stream, (flags & GGUFB200_DEQUANT_SRC_STABLE) != 0);
+}
+
+int ggufb200_quantize(int ggml_type, const void *src, int src_dtype, int64_t n_blocks, void *packed, int flags, void *stream)
+{
+    if (!quantize_supported(ggml_type)) return GGUFB200_E_TYPE;
+    if (flags != 0) return GGUFB200_E_UNSUPPORTED;
+    if (!dtype_ok(src_dtype)) return GGUFB200_E_DTYPE;
+    if (n_blocks < 0) return GGUFB200_E_SHAPE;
+    if (n_blocks == 0) return GGUFB200_OK;
+    if (!src || !packed) return GGUFB200_E_NULL;
+    if (reinterpret_cast<uintptr_t>(src) % (src_dtype == GGUFB200_F32 ? 4 : 2) != 0) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    return quantize_dispatch(ggml_type, src, src_dtype, n_blocks, packed, (cudaStream_t)stream);
 }
 
 int ggufb200_dequant_kron(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,

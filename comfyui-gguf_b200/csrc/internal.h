@@ -39,6 +39,11 @@ int dequant_patched_dora_dispatch(int type, const void *packed, long long N, lon
 int dequant_patched_dispatch(int type, const void *packed, long long N, long long K, void *out, int out_dtype, int math_dtype,
                              const ggufb200_weight_patch *patches, int n_patches, cudaStream_t st);
 
+// quantize.cu, ggufb200_quantize: dense fp32 / fp16 / bf16 -> packed Q4_0 / Q4_1 / Q5_0 / Q5_1 / Q8_0 / BF16; arguments validated by
+// the caller (api.cu)
+bool quantize_supported(int type);
+int quantize_dispatch(int type, const void *src, int src_dtype, long long n_blocks, void *packed, cudaStream_t st);
+
 // ------------------------------------------------------------------ small-M Linear: gemv.cu (GGUFB200_ALGO_GEMV), gemv2.cu (GEMV_FAST)
 int gemv_max_m();
 int gemv_dispatch(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype, int math_dtype,

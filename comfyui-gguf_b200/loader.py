@@ -9,7 +9,9 @@ rebuild gguf_tekken_tokenizer_loader loader.py:334-375, and the sibling mmproj v
 gguf_mmproj_loader loader.py:213-284.  Everything here runs once at load time; the tensors it dequantises go through
 dequantize_tensor (the GPU kernels), and everything it leaves packed runs on the packed-Linear routes.
 
-Out of scope here (SURVEY.md 2, row 9): the sd.cpp "compat" architecture sniffing (needs tools/convert.py).
+Image-model files without `general.architecture`, or with the old `pig` / `cow` tags (stable-diffusion.cpp and early
+converters), load in the reference's compatibility mode (loader.py:77-94, 111-115): the architecture is recognised from the
+tensor names by convert.py's table, and sd.cpp SDXL files get their `proj_in` / `proj_out` shapes fixed.
 """
 from __future__ import annotations
 
@@ -23,6 +25,7 @@ import warnings
 import gguf
 import torch
 
+from .convert import detect_arch
 from .dequant import dequantize_tensor, is_quantized
 from .ops import GGMLTensor
 
@@ -80,17 +83,25 @@ def get_orig_shape(reader, tensor_name):
     return torch.Size(int(field.parts[i][0]) for i in field.data)
 
 
-def _check_arch(arch, kind, is_text_model, path):
+def _check_arch(arch, kind, is_text_model, path, keys):
+    """(architecture, compatibility mode or None).  Image models without an architecture field, or tagged `pig` / `cow`, are
+    recognised from their (prefix-stripped) tensor names: compatibility mode "sd.cpp" or the tag."""
     if arch in (None, "pig", "cow"):
         if is_text_model:
             raise ValueError(f"This gguf file is incompatible with llama.cpp!\nConsider using safetensors or a compatible gguf file\n({path})")
-        raise NotImplementedError("stable-diffusion.cpp style files without general.architecture need the converter's "
-                                  "architecture sniffing, which is outside this package's scope")
+        compat = "sd.cpp" if arch is None else arch
+        try:
+            arch = detect_arch(keys).name
+        except ValueError as e:
+            raise ValueError(f"This model is not currently supported - ({e})") from None
+        logging.warning(f"Warning: This gguf model file is loaded in compatibility mode '{compat}' [arch:{arch}]")
+        return arch, compat
     if is_text_model:
         if arch not in TXT_ARCH_LIST and kind not in VIS_TYPE_LIST:
             raise ValueError(f"Unexpected text model architecture type in GGUF file: {arch!r}")
     elif arch not in IMG_ARCH_LIST:
         raise ValueError(f"Unexpected architecture type in GGUF file: {arch!r}")
+    return arch, None
 
 
 def gguf_sd_loader(path, handle_prefix="model.diffusion_model.", return_arch=False, is_text_model=False):
@@ -103,7 +114,7 @@ def gguf_sd_loader(path, handle_prefix="model.diffusion_model.", return_arch=Fal
         entries = [(name[cut:], t) for name, t in entries if name.startswith(handle_prefix)]
 
     arch = _string_field(reader, "general.architecture")
-    _check_arch(arch, _string_field(reader, "general.type"), is_text_model, path)
+    arch, compat = _check_arch(arch, _string_field(reader, "general.type"), is_text_model, path, [name for name, _ in entries])
 
     state_dict, histogram = {}, {}
     for key, t in entries:
@@ -113,6 +124,10 @@ def gguf_sd_loader(path, handle_prefix="model.diffusion_model.", return_arch=Fal
         shape = get_orig_shape(reader, t.name)
         if shape is None:
             shape = torch.Size(int(v) for v in reversed(t.shape))
+            if compat == "sd.cpp" and arch == "sdxl" and t.name.endswith((".proj_in.weight", ".proj_out.weight")):
+                # sd.cpp writes SDXL's 1x1 projections with their conv shape: drop the trailing size-1 dimensions
+                while len(shape) > 2 and shape[-1] == 1:
+                    shape = shape[:-1]
         if t.tensor_type in (_Q.F32, _Q.F16):
             payload = payload.view(*shape)
         item = GGMLTensor(payload, tensor_type=t.tensor_type, tensor_shape=shape)

@@ -57,6 +57,7 @@ extern "C" {
 #define GGUFB200_OP_ROWS 2
 #define GGUFB200_OP_LINEAR_MMA 3 /* large-M tensor-core path (fused or dequant+GEMM) available for this type */
 #define GGUFB200_OP_DEQUANT_FALLBACK 4 /* ggufb200_dequant_fallback() serves this type */
+#define GGUFB200_OP_QUANTIZE 5 /* ggufb200_quantize() produces this type */
 
 /* algorithm selector for ggufb200_linear(): one GGUFB200_ALGO_* value, optionally OR-ed with GGUFB200_FLAG_* bits */
 #define GGUFB200_ALGO_AUTO 0
@@ -254,6 +255,24 @@ typedef struct ggufb200_dora_patch {
 } ggufb200_dora_patch;
 int ggufb200_dequant_patched_dora(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,
                                   const ggufb200_weight_patch *patches, const ggufb200_dora_patch *dora, int n_patches, void *stream);
+
+/*
+ * Quantise dense values into packed GGUF blocks: the inverse of ggufb200_dequant, used to write GGUF files.  Replaces
+ * gguf-py's `gguf.quants.quantize(values, qtype)` (gguf/quants.py, the Q4_0 ... Q8_0 and BF16 classes) for
+ * Q4_0=2 Q4_1=3 Q5_0=6 Q5_1=7 Q8_0=8 BF16=30.  The source values are widened exactly to fp32; for every finite source the output
+ * is bit-identical to gguf-py's bytes (BF16: for every source, NaN quieting included).  Any other ggml_type: GGUFB200_E_TYPE;
+ * ggufb200_supported(t, GGUFB200_OP_QUANTIZE) lists exactly these six.
+ *   src        n_blocks * block_size contiguous values of src_dtype (0 fp16 / 1 bf16 / 2 fp32), aligned to one value
+ *              (GGUFB200_E_ALIGN otherwise)
+ *   n_blocks   blocks to write (BF16: elements, its block size is 1)
+ *   packed     n_blocks * type_size bytes, block b from src[b*block_size .. +block_size), any alignment
+ *   flags      0; any other bit: GGUFB200_E_UNSUPPORTED (reserved)
+ * The kernels are launched with programmatic stream serialization and execute griddepcontrol.launch_dependents only after
+ * their last write of `packed`, so a following ggufb200_dequant with GGUFB200_DEQUANT_SRC_STABLE, or a ggufb200_linear with
+ * GGUFB200_FLAG_W_STABLE, on the same stream may consume the packed bytes without any other synchronisation.
+ *   stream     a cudaStream_t, as everywhere in this header
+ */
+int ggufb200_quantize(int ggml_type, const void *src, int src_dtype, int64_t n_blocks, void *packed, int flags, void *stream);
 
 /*
  * Integer unpack only (test/debug surface for the "bit-exact integer unpack" contract):
