@@ -20,7 +20,7 @@ ALGO_MASK = 0xFF
 FLAG_EXACT_W, FLAG_GENERIC, FLAG_TILE384, FLAG_NOSPLIT, FLAG_UNSTAGED, FLAG_TILE192 = 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000
 FLAG_W_STABLE = 0x4000          # ggufb200_linear: no kernel still in flight writes the packed weight (prefetch under the previous kernel's tail)
 DEQUANT_SRC_STABLE = 0x100      # same promise for ggufb200_dequant, OR-ed into math_dtype
-OP_DEQUANT, OP_LINEAR, OP_ROWS, OP_LINEAR_MMA, OP_DEQUANT_FALLBACK, OP_QUANTIZE = 0, 1, 2, 3, 4, 5
+OP_DEQUANT, OP_LINEAR, OP_ROWS, OP_LINEAR_MMA, OP_DEQUANT_FALLBACK, OP_QUANTIZE, OP_LINEAR_GRAD = 0, 1, 2, 3, 4, 5, 6
 LOWRANK_MAX_PATCHES, LOWRANK_MAX_RANK = 8, 1024   # ggufb200_dequant_lowrank: descriptors per call, rank of one factor pair
 PATCH_LOWRANK, PATCH_KRON = 0, 1                   # ggufb200_weight_patch.kind
 DORA_AXIS_OUT, DORA_AXIS_IN = 0, 1                 # ggufb200_dora_patch.axis
@@ -113,6 +113,9 @@ def lib() -> ctypes.CDLL:
                                               c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_sz, c_int, c_vp]
     L.ggufb200_gemm_scaled.argtypes = [c_vp, c_i64, c_i64, c_i64, c_vp, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_vp, c_i64, c_vp]
     L.ggufb200_scale_columns.argtypes = [c_vp, c_i64, c_i64, c_i64, c_int, c_vp, c_vp, c_i64, c_vp]
+    L.ggufb200_linear_grad_input_workspace.restype = c_sz
+    L.ggufb200_linear_grad_input_workspace.argtypes = [c_int, c_i64, c_i64, c_int]
+    L.ggufb200_linear_grad_input.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_int, c_int, c_vp, c_i64, c_vp, c_sz, c_int, c_vp]
     _lib = L
     return L
 
@@ -129,5 +132,5 @@ EXPORTS = (
     "ggufb200_repack_bytes", "ggufb200_repack", "ggufb200_linear_spans", "ggufb200_linear_lora",
     "ggufb200_linear_lora_ex", "ggufb200_dequant_kron", "ggufb200_dequant_fallback", "ggufb200_linear_lora_scaled",
     "ggufb200_gemm_scaled", "ggufb200_scale_columns", "ggufb200_dequant_lowrank", "ggufb200_dequant_patched",
-    "ggufb200_dequant_patched_dora", "ggufb200_quantize",
+    "ggufb200_dequant_patched_dora", "ggufb200_quantize", "ggufb200_linear_grad_input_workspace", "ggufb200_linear_grad_input",
 )

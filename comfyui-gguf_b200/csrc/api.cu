@@ -28,6 +28,18 @@ static bool dtype_ok(int d) { return d >= 0 && d <= 2; }
 static bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 static bool fused_type(int t) { return t != T_BF16 && type_geom(t, nullptr, nullptr); }     // every block format has a fused producer
 
+// the types ggufb200_linear_grad_input dequantises: the table (ggufb200_dequant) and the numpy-fallback types
+static bool grad_type(int t, int *bs)
+{
+    int b = 0;
+    const bool known = type_geom(t, &b, nullptr) || with_fallback_block(t, false, [&](auto blk) {
+        b = decltype(blk)::BS;
+        return true;
+    });
+    if (known && bs) *bs = b;
+    return known;
+}
+
 // ------------------------------------------------------------------ device gate
 // The library contains sm_90a code only.  Checked once per device, right before the first launch on it (argument
 // errors are still reported without a GPU).
@@ -149,6 +161,7 @@ int ggufb200_supported(int ggml_type, int op)
 {
     if (op == GGUFB200_OP_DEQUANT_FALLBACK) return with_fallback_block(ggml_type, 0, [](auto) { return 1; });
     if (op == GGUFB200_OP_QUANTIZE) return quantize_supported(ggml_type) ? 1 : 0;
+    if (op == GGUFB200_OP_LINEAR_GRAD) return grad_type(ggml_type, nullptr) ? 1 : 0;
     if (!type_geom(ggml_type, nullptr, nullptr)) return 0;
     switch (op) {
     case GGUFB200_OP_DEQUANT: return 1;
@@ -565,6 +578,55 @@ int ggufb200_gemm_scaled(const void *W, int64_t N, int64_t K, int64_t ldw, const
     if (feature_scale && !aligned16(feature_scale)) return GGUFB200_E_ALIGN;
     if (int rc = device_check()) return rc;
     return dense_gemm(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, (cudaStream_t)stream, feature_scale);
+}
+
+// BF16 weight, bf16 activations: W's bytes are already the operand
+static bool grad_reads_in_place(int ggml_type, int act_dtype) { return ggml_type == T_BF16 && act_dtype == kBF16; }
+
+size_t ggufb200_linear_grad_input_workspace(int ggml_type, int64_t N, int64_t K, int act_dtype)
+{
+    if (!grad_type(ggml_type, nullptr) || N <= 0 || K <= 0 || grad_reads_in_place(ggml_type, act_dtype)) return 0;
+    return (size_t)N * (size_t)K * 2;
+}
+
+int ggufb200_linear_grad_input(int ggml_type, const void *W_packed, int64_t N, int64_t K, const void *dY, int64_t M, int64_t ldy, int act_dtype,
+                               int math_dtype, void *dX, int64_t ldx, void *workspace, size_t workspace_bytes, int flags, void *stream)
+{
+    int bs = 0;
+    if (!grad_type(ggml_type, &bs)) return GGUFB200_E_TYPE;
+    if (act_dtype != kF16 && act_dtype != kBF16) return GGUFB200_E_DTYPE;
+    if (!dtype_ok(math_dtype)) return GGUFB200_E_DTYPE;
+    if (flags & ~GGUFB200_FLAG_W_STABLE) return GGUFB200_E_UNSUPPORTED;
+    const bool fallback = !type_geom(ggml_type, nullptr, nullptr);
+    if (M < 0 || N <= 0 || K <= 0 || K % 8 != 0 || ldy < N || ldx < K || (N * K) % bs != 0) return GGUFB200_E_SHAPE;
+    if (!fallback && K % bs != 0 && !straddled_rows(bs, N, K)) return GGUFB200_E_SHAPE;
+    if (M == 0) return GGUFB200_OK;
+    if (!W_packed || !dY || !dX) return GGUFB200_E_NULL;
+    if (!aligned16(dY) || !aligned16(dX) || (ldy % 8) || (ldx % 8)) return GGUFB200_E_ALIGN;
+    const bool in_place = grad_reads_in_place(ggml_type, act_dtype);
+    if (in_place && !aligned16(W_packed)) return GGUFB200_E_ALIGN;
+    const size_t dense = in_place ? 0 : (size_t)N * (size_t)K * 2;
+    if (dense && (!workspace || workspace_bytes < dense)) return GGUFB200_E_WORKSPACE;
+    if (dense && !aligned16(workspace)) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    // An autograd backward runs on a worker thread that may have no current context yet; the first launch of a kernel instance
+    // raises its shared-memory limit (cudaFuncSetAttribute), which fails there.  cudaSetDevice binds the primary context.
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaSetDevice(dev) != cudaSuccess) {
+        cudaGetLastError();
+        return GGUFB200_E_CUDA;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    const bool stable = (flags & GGUFB200_FLAG_W_STABLE) != 0;
+    const void *W = W_packed;
+    if (!in_place) {
+        const long long n_blocks = N * K / bs;
+        const int rc = fallback ? fallback_dispatch(ggml_type, W_packed, n_blocks, workspace, act_dtype, st, stable)
+                                : dequant_dispatch(ggml_type, W_packed, n_blocks, workspace, act_dtype, math_dtype, st, stable);
+        if (rc != GGUFB200_OK) return rc;
+        W = workspace;
+    }
+    return dense_gemm_nn(W, N, K, K, dY, M, ldy, act_dtype, dX, ldx, st);
 }
 
 int ggufb200_scale_columns(const void *X, int64_t M, int64_t K, int64_t ldx, int act_dtype, const float *col_scale, void *Y, int64_t ldy,

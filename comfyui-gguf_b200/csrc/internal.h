@@ -80,6 +80,10 @@ struct LinearOptions {
 // scale: nullptr, or fp32 [N] (16-byte aligned) multiplied into each output feature before the bias (ggufb200_gemm_scaled).
 int dense_gemm(const void *W, long long N, long long K, long long ldw, const void *X, long long M, long long ldx, int act_dtype,
                const void *bias, int bias_dtype, void *Y, long long ldy, cudaStream_t st, const float *scale = nullptr);
+// Y[M, Kout] = X[M, Nred] * B[Nred, Kout] with B row-major (ldb >= Kout), fp32 accumulation, no bias: the GEMM of
+// ggufb200_linear_grad_input.  Kout % 8 == 0; the alignment rules of dense_gemm.
+int dense_gemm_nn(const void *B, long long Nred, long long Kout, long long ldb, const void *X, long long M, long long ldx, int act_dtype, void *Y,
+                  long long ldy, cudaStream_t st);
 // GGUFB200_ALGO_FUSED_MMA: reference-exact producers, the weight as the wide operand.
 size_t fused_mma_workspace(long long M, long long N, long long K, const LinearOptions &opt);
 void fused_mma_plan(long long M, long long N, long long K, size_t ws_bytes, const LinearOptions &opt, int *tile_rows, int *splits,

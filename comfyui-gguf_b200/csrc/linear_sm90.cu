@@ -5,6 +5,8 @@
 //
 //   dense_gemm          W dense: both operands TMA-fed, one CTA per 128-token x BN-feature tile (ggufb200_gemm and the GEMM
 //                       half of GGUFB200_ALGO_DEQUANT_MMA).  A ragged last k-block is zero-filled by the TMA engine.
+//   dense_gemm_nn       Y[M, Kout] = X[M, Nred] * B[Nred, Kout], B row-major (ggufb200_linear_grad_input: dX = dY * W with the
+//                       dequantised W): the same kernel and tiling with B staged MN-major straight from its rows (B_MN).
 //   fused_mma_linear    GGUFB200_ALGO_FUSED_MMA: A = 128 activation rows (TMA), B = 256 weight rows that the producer warpgroup
 //                       dequantises from the canonical packed rows with the reference's fp16 rounding sequence (Producer<Q>),
 //                       so the weight operand is bit-identical to what the reference hands to F.linear.  Every block format,
@@ -96,6 +98,36 @@ int dense_gemm(const void *W, long long N, long long K, long long ldw, const voi
     if (K % 8 != 0 || N % 8 != 0) return GGUFB200_E_UNSUPPORTED;
     return scale ? dense_tiles<true>(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st, scale)
                  : dense_tiles<false>(W, N, K, ldw, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st, nullptr);
+}
+
+template <int ACT, int BN>
+static int dense_nn_launch(const void *B, long long Nred, long long Kout, long long ldb, const void *X, long long M, long long ldx, void *Y,
+                           long long ldy, cudaStream_t st)
+{
+    CUtensorMap tmA, tmB;
+    if (!make_kblock_map(&tmA, X, M, Nred, ldx, ACT, 128)) return GGUFB200_E_CUDA;
+    if (!make_kblock_map(&tmB, B, Nred, Kout, ldb, ACT, 64)) return GGUFB200_E_CUDA;      // [64 k rows][64 columns] boxes
+    WgParams p{};
+    p.M = M; p.N = Kout; p.K = Nred;
+    p.Y = reinterpret_cast<uint8_t *>(Y); p.ldy = ldy;
+    p.ttiles = (int)((M + 127) / 128);
+    p.ftiles = (int)((Kout + BN - 1) / BN);
+    p.kb_total = (int)((Nred + kBlockK - 1) / kBlockK);
+    p.kb_per_split = p.kb_total;
+    return wg_launch<void, void, ACT, BN, false, false, false, true>(tmA, tmB, tmA, p, 1, st);
+}
+
+int dense_gemm_nn(const void *B, long long Nred, long long Kout, long long ldb, const void *X, long long M, long long ldx, int act_dtype, void *Y,
+                  long long ldy, cudaStream_t st)
+{
+    if (Kout % 8 != 0) return GGUFB200_E_UNSUPPORTED;
+    // output tiles as dense_tiles: 256 columns wide, 128 when that leaves most SMs idle
+    const bool narrow = ((M + 127) / 128) * ((Kout + 255) / 256) < sm_count();
+    if (narrow)
+        return act_dtype == kBF16 ? dense_nn_launch<kBF16, 128>(B, Nred, Kout, ldb, X, M, ldx, Y, ldy, st)
+                                  : dense_nn_launch<kF16, 128>(B, Nred, Kout, ldb, X, M, ldx, Y, ldy, st);
+    return act_dtype == kBF16 ? dense_nn_launch<kBF16, 256>(B, Nred, Kout, ldb, X, M, ldx, Y, ldy, st)
+                              : dense_nn_launch<kF16, 256>(B, Nred, Kout, ldb, X, M, ldx, Y, ldy, st);
 }
 
 // ------------------------------------------------------------------ GGUFB200_ALGO_FUSED_MMA

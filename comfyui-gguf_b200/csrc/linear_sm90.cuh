@@ -19,6 +19,9 @@
 // rounds to the activation dtype and writes the tile through shared memory with 16-byte stores.  SCALED instances first
 // multiply each output feature by an fp32 factor: Y = act(scale[n] * acc + bias[n]) (DoRA's row norms, ggufb200_*_scaled);
 // a template parameter, so that the unscaled instances are compiled exactly as without it.
+// B_MN (dense, TRANS = false only): the weight operand is a row-major [K, N] matrix B, Y = X * B, read MN-major: each stage's
+// B tile is TN / 64 TMA boxes of [64 k rows][64 columns] straight from B's rows, and wgmma's transpose bit reads them (the
+// input gradient dX = dY * W of ggufb200_linear_grad_input, W never transposed in memory).
 #pragma once
 #include <type_traits>
 
@@ -74,7 +77,7 @@ template <int ACT> __device__ __forceinline__ uint32_t wg_h2_to_act(uint32_t h)
     }
 }
 
-template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false, bool SCALED = false>
+template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false, bool SCALED = false, bool B_MN = false>
 __global__ void __launch_bounds__(kWgThreads, 1)
 wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmT,
                  const WgParams p)
@@ -83,6 +86,7 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     constexpr bool DENSE = std::is_same<Prod, void>::value;
     constexpr int STAGES = Cfg::STAGES, TOK = Cfg::TOK, FEAT = Cfg::FEAT;
     constexpr int WROWS = TRANS ? 128 : TN;                   // weight rows of a stage
+    static_assert(!B_MN || (DENSE && !TRANS && TN % 64 == 0), "MN-major B: dense GEMM, token x feature orientation");
 
     const int per = p.ftiles * p.ttiles;
     const int split = blockIdx.x / per;
@@ -135,7 +139,12 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
             if (t == 0) {
                 mbar_arrive_expect_tx(&full[s], TOK * 128 + (DENSE ? WROWS * 128 : 0));
                 tma_load_2d(x_tile, lora_kb ? &tmT : &tmX, &full[s], lora_kb ? lj * kBlockK : kb * kBlockK, (int)tok0);
-                if constexpr (DENSE) tma_load_2d(w_tile, &tmW, &full[s], kb * kBlockK, (int)feat0);
+                if constexpr (DENSE && B_MN) {
+#pragma unroll
+                    for (int c = 0; c < TN / 64; ++c) tma_load_2d(w_tile + c * 64 * 128, &tmW, &full[s], (int)feat0 + 64 * c, kb * kBlockK);
+                } else if constexpr (DENSE) {
+                    tma_load_2d(w_tile, &tmW, &full[s], kb * kBlockK, (int)feat0);
+                }
             }
             if constexpr (!DENSE) {
 #pragma unroll 1
@@ -196,10 +205,17 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         mbar_wait(&full[s], (uint32_t)((i / STAGES) & 1));
         const uint32_t a_addr = base + (uint32_t)(s * Cfg::STAGE) + (uint32_t)(cw * 64 * 128);
         const uint32_t b_addr = base + (uint32_t)(s * Cfg::STAGE + Cfg::A_BYTES);
-        const uint64_t da = wg_desc_sw128(a_addr), db = wg_desc_sw128(b_addr);
+        const uint64_t da = wg_desc_sw128(a_addr);
         wgmma_fence();
+        if constexpr (B_MN) {
+            const uint64_t db = wg_desc_sw128_mn(b_addr);
 #pragma unroll
-        for (int j = 0; j < kBlockK / 16; ++j) Wgmma<ACT, TN>::mma(acc, da + (uint64_t)(2 * j), db + (uint64_t)(2 * j));
+            for (int j = 0; j < kBlockK / 16; ++j) Wgmma<ACT, TN>::template mma<1>(acc, da + (uint64_t)(2 * j), db + (uint64_t)(128 * j));
+        } else {
+            const uint64_t db = wg_desc_sw128(b_addr);
+#pragma unroll
+            for (int j = 0; j < kBlockK / 16; ++j) Wgmma<ACT, TN>::mma(acc, da + (uint64_t)(2 * j), db + (uint64_t)(2 * j));
+        }
         wgmma_commit();
         if (i > 0) {
             wgmma_wait<1>();                                   // k-block i-1 has been read: hand its stage back
@@ -260,11 +276,11 @@ wg_linear_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
 }
 
 // Launch one CTA per (split, feature tile, token tile).  tmT: LoRA T tile map (or a copy of tmX).
-template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false, bool SCALED = false>
+template <class Q, class Prod, int ACT, int TN, bool TRANS, bool STRADDLED = false, bool SCALED = false, bool B_MN = false>
 static int wg_launch(const CUtensorMap &tmX, const CUtensorMap &tmW, const CUtensorMap &tmT, const WgParams &p, int splits, cudaStream_t st)
 {
     using Cfg = WgCfg<TN, TRANS>;
-    auto kern = wg_linear_kernel<Q, Prod, ACT, TN, TRANS, STRADDLED, SCALED>;
+    auto kern = wg_linear_kernel<Q, Prod, ACT, TN, TRANS, STRADDLED, SCALED, B_MN>;
     static unsigned char attr[64] = {};
     if (!ensure_dynamic_smem(kern, Cfg::SMEM, attr)) return GGUFB200_E_CUDA;
     const long long ctas = (long long)p.ftiles * p.ttiles * splits;

@@ -13,6 +13,10 @@ What changes underneath:
       then comfy.lora.calculate_weight / F.linear) so their semantics stay those of the reference.
     * get_weight (ops.py:166-191) dequantises with ONE kernel launch (dequant.py of this package).
     * Embedding (ops.py:251-259) gathers only the indexed rows instead of dequantising the whole table.
+    * The packed-weight Linear is differentiable in its input like the reference's F.linear (`grad_needed`,
+      PackedLinearFunction): the backward dequantises W again from the packed bytes (ggufb200_linear_grad_input) instead of
+      keeping a dense W per layer between forward and backward; patch lists other than plain / banded LoRA, and patched
+      Conv2d weights, take the two-step route while gradients are needed.
 """
 from __future__ import annotations
 
@@ -279,6 +283,82 @@ def linear_dense(x, weight, bias=None, feature_scale=None):
                                                  torch.cuda.current_stream(x.device).cuda_stream)
     _lib.check(rc, f"ggufb200_gemm(M={M}, N={N}, K={K})")
     return y.reshape(*x.shape[:-1], N)
+
+
+def linear_grad_input(dy, wraw, qtype, N, K, math):
+    """dX = dY @ W for a CUDA fp16/bf16 dY [..., N] and the packed rows `wraw` (plain uint8 on dy.device) of an [N, K] weight
+    (ggufb200_linear_grad_input): W is dequantised with the math dtype code `math` into a workspace, never kept."""
+    dy2 = dy.reshape(-1, N)
+    # rows that overlap (a stride below N: autograd hands broadcast gradients such as that of y.sum(0) with row stride 0), are
+    # not contiguous, or do not start on 16-byte boundaries are copied
+    if dy2.stride(-1) != 1 or dy2.stride(0) < N or (dy2.stride(0) % 8) != 0 or (dy2.data_ptr() % 16) != 0:
+        pad = -N % 8                                     # rows of dY must start on 16-byte boundaries: pad them to 8 elements
+        dy2 = torch.nn.functional.pad(dy2, (0, pad)) if pad else dy2.contiguous()
+    if not wraw.is_contiguous() or (qtype == _Q.BF16 and wraw.data_ptr() & 15):      # BF16 rows are read in place: 16-byte aligned
+        wraw = wraw.clone(memory_format=torch.contiguous_format)
+    M = dy2.shape[0]
+    dx = torch.empty(M, K, dtype=dy.dtype, device=dy.device)
+    L = _lib.lib()
+    qcode, act = int(qtype), dtype_code(dy.dtype)
+    need = L.ggufb200_linear_grad_input_workspace(qcode, N, K, act)
+    ws = torch.empty(need, dtype=torch.uint8, device=dy.device) if need else None
+    with torch.cuda.device(dy.device):
+        rc = L.ggufb200_linear_grad_input(qcode, wraw.data_ptr(), N, K, dy2.data_ptr(), M, dy2.stride(0), act, math, dx.data_ptr(), K,
+                                          None if ws is None else ws.data_ptr(), need, _lib.FLAG_W_STABLE,
+                                          _current_stream_ptr(dy.device.index))
+    _lib.check(rc, f"ggufb200_linear_grad_input({getattr(qtype, 'name', qtype)}, M={M}, N={N}, K={K})")
+    return dx.reshape(*dy.shape[:-1], K)
+
+
+class PackedLinearFunction(torch.autograd.Function):
+    """y = run(), the packed-weight Linear's forward as it runs without gradients (bit-identical output), differentiable in x.
+
+    Saves only the packed rows `wraw` and the (qtype, N, K, math) metadata, never a dense W: the backward dequantises again
+    from the packed bytes (`linear_grad_input`).  The weight and bias are frozen (no gradient).  The backward always uses the
+    exact weight, also after a `fast`-contract forward.  Once differentiable: double backward raises."""
+
+    @staticmethod
+    def forward(ctx, x, wraw, run, qtype, N, K, math):
+        ctx.save_for_backward(wraw)
+        ctx.meta = (qtype, N, K, math)
+        return run()
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dy):
+        (wraw,) = ctx.saved_tensors
+        dx = linear_grad_input(dy, wraw, *ctx.meta) if ctx.needs_input_grad[0] else None
+        return dx, None, None, None, None, None, None
+
+
+def _requires_grad(item):
+    """True when a tensor inside a patch structure (entries, payload tuples, adapter objects' `.weights`) requires grad."""
+    if torch.is_tensor(item):
+        return item.requires_grad
+    if isinstance(item, (tuple, list)):
+        return any(_requires_grad(x) for x in item)
+    weights = getattr(item, "weights", None)
+    return weights is not None and _requires_grad(weights)
+
+
+def grad_needed(input, weight):
+    """The one predicate of the differentiable routes: gradients are being recorded and the input or a factor of the weight's
+    patches requires grad.  False keeps every route, launch and output bit exactly as without autograd."""
+    return torch.is_grad_enabled() and (input.requires_grad or _requires_grad(getattr(weight, "patches", ())))
+
+
+def lora_side_sum(y, x, terms):
+    """y + sum of the LoRA side terms scale * (x_band down^T) up^T of `lora_band_terms`, in differentiable torch ops (gradients
+    reach x, up and down with calculate_weight's scale strength * alpha / r); a row band adds into its output columns only."""
+    N = y.shape[-1]
+    for scale, up, down, band in terms:
+        xs = x[..., band[1]:band[1] + band[2]] if band is not None and band[0] == 1 else x
+        u = (up.to(device=x.device, dtype=torch.float32) * scale).to(x.dtype)
+        t = torch.nn.functional.linear(torch.nn.functional.linear(xs, down.to(device=x.device, dtype=x.dtype)), u)
+        if band is not None and band[0] == 0:
+            t = torch.nn.functional.pad(t, (band[1], N - band[1] - band[2]))
+        y = y + t
+    return y
 
 
 def scale_columns(x, col_scale):
@@ -1399,16 +1479,21 @@ class GGMLOps(comfy_ops.manual_cast):
             return (self.lora_in_kernel and math == _F16_CODE and N % 8 == 0 and qtype != _Q.BF16 and qtype not in FALLBACK_QTYPES
                     and (spans is not None or not needs_span_layout(qtype, K)))
 
+        # Autograd (`grad_needed`): an unpatched weight keeps the route it takes without gradients, wrapped in
+        # PackedLinearFunction (same output bits; the backward is ggufb200_linear_grad_input on the packed bytes, no dense W is
+        # saved); a plain or banded LoRA list takes that base plus its side terms in torch ops (`lora_side_sum`, gradients for x,
+        # up and down); every other patch list takes the two-step route, the reference's own differentiable arithmetic.
         def forward_ggml_cast_weights(self, input):
             y = None
             if self._fused_ok(input):
                 dev = input.device
+                grad = grad_needed(input, self.weight)
                 terms, kron, dora = self._lora_terms(dev), None, None
-                if terms is None and self.weight.tensor_type not in FALLBACK_QTYPES:
+                if terms is None and self.weight.tensor_type not in FALLBACK_QTYPES and not grad:
                     lycoris = self._lycoris_terms(dev)                 # LoHa / LoKr entries: LoRA terms + LoKr patches
                     if lycoris is not None:
                         terms, kron = lycoris
-                if terms is None:
+                if terms is None and not grad:
                     dora = self._dora_terms()                          # tried after the LoRA and LyCORIS recognisers declined
                 if terms is not None or dora is not None:
                     w = self.weight
@@ -1422,6 +1507,7 @@ class GGMLOps(comfy_ops.manual_cast):
                         if b.device != dev:
                             b = b.to(dev)
                     M = input.numel() // K if input.shape[-1] == K else -1
+                    run = None                                         # the unpatched forward, where a kernel route serves it
                     if M < 0:
                         pass                                           # feature mismatch: let F.linear raise the usual error
                     elif dora is not None:
@@ -1431,15 +1517,16 @@ class GGMLOps(comfy_ops.manual_cast):
                         # numpy-fallback types (csrc/fallback.cuh): no fused kernel reads them, so K1 into an [N, K] activation-dtype
                         # weight (the reference's fp32 -> dtype rounding) + the dense GEMM at every M; other shapes: two-step route
                         if N % 8 == 0 and K % 8 == 0:
-                            W = dequantize_fallback(wraw, qtype, (N, K), input.dtype)
-                            y = linear_dense(input, W, b)
+                            def run():
+                                return linear_dense(input, dequantize_fallback(wraw, qtype, (N, K), input.dtype), b)
                     elif kron is not None:
                         # LoKr: the patched weight in one K1 launch + the dense GEMM at every M; LoRA / LoHa terms as side GEMMs
                         if qtype != _Q.BF16 and N % 8 == 0 and K % 8 == 0 and len(kron[0]) <= KRON_MAX_PATCHES:
                             y = self._kron_linear(input, wraw, qtype, N, K, b, kron)
                     elif qtype == _Q.BF16 and M > GEMV_MAX_M:
                         if input.dtype == torch.bfloat16 and K % 8 == 0 and N % 8 == 0:   # already dense: straight to the tensor-core GEMM
-                            y = linear_dense(input, wraw.view(torch.bfloat16).view(N, K), b)
+                            def run():
+                                return linear_dense(input, wraw.view(torch.bfloat16).view(N, K), b)
                     elif M <= GEMV_MAX_M or N % 8 == 0:                # (the M <= 8 kernel stores per element: any N)
                         math = math_code(self.dequant_dtype, input.dtype)
                         # W_STABLE: the packed weight is a parameter (or its host-to-device copy just above): never written by a
@@ -1449,15 +1536,21 @@ class GGMLOps(comfy_ops.manual_cast):
                         if self._takes_span_copy(qtype, N, K, M, math, resident):
                             spans = span_layout(w, wraw)               # cached on the tensor after the first forward
                             algo = _lib.ALGO_FUSED_TMEM | exact
-                        lora = None
-                        if (terms and self._takes_lora_kblocks(qtype, N, K, math, spans)
+                        if (terms and not grad and self._takes_lora_kblocks(qtype, N, K, math, spans)
                                 and sum(d.shape[0] for _s, _u, d, _b in terms) <= LORA_KERNEL_MAX_RANK):
                             down_pad, u_pad, tiles = self._lora_operands(terms, dev, input.dtype)
                             lora = (linear_dense(input.reshape(-1, K), down_pad), u_pad, tiles)       # T = x * down^T, [M, 64 J]
-                            algo = _lib.ALGO_FUSED_TMEM | exact
-                        y = _launch_linear(input, wraw, qtype, N, K, b, math, algo, spans, lora)
-                        if lora is not None:
-                            return y
+                            return _launch_linear(input, wraw, qtype, N, K, b, math, _lib.ALGO_FUSED_TMEM | exact, spans, lora)
+
+                        def run():
+                            return _launch_linear(input, wraw, qtype, N, K, b, math, algo, spans)
+                    if run is not None:
+                        if not grad:
+                            y = run()
+                        else:
+                            math = math_code(self.dequant_dtype, input.dtype)
+                            y = PackedLinearFunction.apply(input, wraw, run, qtype, N, K, math)
+                            return lora_side_sum(y, input, terms) if terms else y
                     if y is not None and terms:
                         y = self._add_lora(y, input, terms)
             if y is not None:
@@ -1552,6 +1645,9 @@ class GGMLOps(comfy_ops.manual_cast):
             return _cached(self, "_gg_conv_dora_" + str(dtype).split(".")[-1], key, build)
 
         def forward_ggml_cast_weights(self, input):
+            if grad_needed(input, self.weight):                       # the patch kernels' weight carries no gradient
+                weight, bias = self.cast_bias_weight(input)
+                return self._conv_forward(input, weight, bias)
             entry, operands = "ggufb200_dequant_lowrank", self._conv_patch_operands(input)
             if operands is None:
                 entry, operands = "ggufb200_dequant_patched", self._conv_lycoris_operands(input)

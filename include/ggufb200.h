@@ -58,6 +58,7 @@ extern "C" {
 #define GGUFB200_OP_LINEAR_MMA 3 /* large-M tensor-core path (fused or dequant+GEMM) available for this type */
 #define GGUFB200_OP_DEQUANT_FALLBACK 4 /* ggufb200_dequant_fallback() serves this type */
 #define GGUFB200_OP_QUANTIZE 5 /* ggufb200_quantize() produces this type */
+#define GGUFB200_OP_LINEAR_GRAD 6 /* ggufb200_linear_grad_input() serves this type */
 
 /* algorithm selector for ggufb200_linear(): one GGUFB200_ALGO_* value, optionally OR-ed with GGUFB200_FLAG_* bits */
 #define GGUFB200_ALGO_AUTO 0
@@ -401,6 +402,28 @@ int ggufb200_gemm(const void *W, int64_t N, int64_t K, int64_t ldw, const void *
  * feature_scale: NULL (ggufb200_gemm, bit for bit) or N floats in device memory, 16-byte aligned (GGUFB200_E_ALIGN). */
 int ggufb200_gemm_scaled(const void *W, int64_t N, int64_t K, int64_t ldw, const void *X, int64_t M, int64_t ldx, int act_dtype,
                          const void *bias, int bias_dtype, const float *feature_scale, void *Y, int64_t ldy, void *stream);
+
+/*
+ * Input gradient of the packed-weight Linear: dX[M, K] = dY[M, N] * W[N, K], W = dequant(W_packed) in act_dtype with the
+ * reference's rounding sequence in math_dtype (the weight the reference's F.linear saves for its backward; the exact contract
+ * whatever the forward ran).  Two steps on `stream`: the standalone dequant (ggufb200_dequant, or ggufb200_dequant_fallback
+ * for its eleven types, which ignore math_dtype) writes W into the workspace, then the dense warpgroup-MMA GEMM reads W's rows
+ * MN-major (no transposed copy), fp32 accumulation.  A BF16 weight with bf16 activations is read as it is: no dequant, no
+ * workspace.
+ *   ggml_type   every type of ggufb200_dequant and of ggufb200_dequant_fallback (ggufb200_supported(t, GGUFB200_OP_LINEAR_GRAD))
+ *   W_packed    the rows as in ggufb200_linear (straddled weights included); for the types of ggufb200_dequant_fallback the
+ *               flat block stream of the [N, K] tensor, N * K a multiple of the block size.  Any alignment, except the BF16 read
+ *               in place (16-byte aligned, GGUFB200_E_ALIGN)
+ *   dY, dX      act_dtype (0 fp16 / 1 bf16), row strides ldy >= N and ldx >= K in ELEMENTS, multiples of 8, 16-byte aligned
+ *               (GGUFB200_E_ALIGN); K % 8 == 0 (GGUFB200_E_SHAPE); any N
+ *   workspace   at least ggufb200_linear_grad_input_workspace() bytes (N * K * 2, or 0), 16-byte aligned
+ *   flags       0 or GGUFB200_FLAG_W_STABLE (passed on to the dequant as GGUFB200_DEQUANT_SRC_STABLE); any other bit:
+ *               GGUFB200_E_UNSUPPORTED
+ */
+size_t ggufb200_linear_grad_input_workspace(int ggml_type, int64_t N, int64_t K, int act_dtype);
+int ggufb200_linear_grad_input(int ggml_type, const void *W_packed, int64_t N, int64_t K, const void *dY, int64_t M, int64_t ldy,
+                               int act_dtype, int math_dtype, void *dX, int64_t ldx, void *workspace, size_t workspace_bytes, int flags,
+                               void *stream);
 
 /*
  * Column scale: Y[m, k] = act(float(X[m, k]) * col_scale[k]) for m < M, k < K, one fp32 multiply and one round-to-nearest
