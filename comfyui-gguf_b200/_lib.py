@@ -15,12 +15,14 @@ _lib = None
 
 F16, BF16, F32 = 0, 1, 2
 ALGO_AUTO, ALGO_GEMV, ALGO_FUSED_MMA, ALGO_DEQUANT_MMA, ALGO_FUSED_TMEM, ALGO_GEMV_FAST = 0, 1, 2, 3, 4, 5
+ALGO_FUSED_SYNC = 6             # ggufb200_linear_fallback only
 ALGO_MASK = 0xFF
 # per-call switches OR-ed into `algo` (include/ggufb200.h)
 FLAG_EXACT_W, FLAG_GENERIC, FLAG_TILE384, FLAG_NOSPLIT, FLAG_UNSTAGED, FLAG_TILE192 = 0x100, 0x200, 0x400, 0x800, 0x1000, 0x2000
 FLAG_W_STABLE = 0x4000          # ggufb200_linear: no kernel still in flight writes the packed weight (prefetch under the previous kernel's tail)
 DEQUANT_SRC_STABLE = 0x100      # same promise for ggufb200_dequant, OR-ed into math_dtype
 OP_DEQUANT, OP_LINEAR, OP_ROWS, OP_LINEAR_MMA, OP_DEQUANT_FALLBACK, OP_QUANTIZE, OP_LINEAR_GRAD = 0, 1, 2, 3, 4, 5, 6
+OP_LINEAR_FALLBACK, OP_ROWS_FALLBACK = 7, 8
 LOWRANK_MAX_PATCHES, LOWRANK_MAX_RANK = 8, 1024   # ggufb200_dequant_lowrank: descriptors per call, rank of one factor pair
 PATCH_LOWRANK, PATCH_KRON = 0, 1                   # ggufb200_weight_patch.kind
 DORA_AXIS_OUT, DORA_AXIS_IN = 0, 1                 # ggufb200_dora_patch.axis
@@ -90,6 +92,11 @@ def lib() -> ctypes.CDLL:
     L.ggufb200_quantize.argtypes = [c_int, c_vp, c_int, c_i64, c_vp, c_int, c_vp]
     L.ggufb200_unpack_int.argtypes = [c_int, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp]
     L.ggufb200_dequant_rows.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_int, c_int, c_vp]
+    L.ggufb200_dequant_rows_fallback.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_i64, c_vp, c_int, c_vp]
+    L.ggufb200_linear_fallback_workspace.restype = c_sz
+    L.ggufb200_linear_fallback_workspace.argtypes = [c_int, c_i64, c_i64, c_i64, c_int, c_int]
+    L.ggufb200_linear_fallback_route.argtypes = [c_int, c_i64, c_i64, c_i64, c_int, c_int]
+    L.ggufb200_linear_fallback.argtypes = [c_int, c_vp, c_i64, c_i64, c_vp, c_i64, c_i64, c_int, c_vp, c_int, c_vp, c_i64, c_vp, c_sz, c_int, c_vp]
     L.ggufb200_linear_plan.restype = c_int
     L.ggufb200_linear_plan.argtypes = [c_int, c_i64, c_i64, c_i64, c_sz, c_int] + [ctypes.POINTER(c_int)] * 4
     L.ggufb200_linear_workspace.restype = c_sz
@@ -133,4 +140,5 @@ EXPORTS = (
     "ggufb200_linear_lora_ex", "ggufb200_dequant_kron", "ggufb200_dequant_fallback", "ggufb200_linear_lora_scaled",
     "ggufb200_gemm_scaled", "ggufb200_scale_columns", "ggufb200_dequant_lowrank", "ggufb200_dequant_patched",
     "ggufb200_dequant_patched_dora", "ggufb200_quantize", "ggufb200_linear_grad_input_workspace", "ggufb200_linear_grad_input",
+    "ggufb200_dequant_rows_fallback", "ggufb200_linear_fallback_workspace", "ggufb200_linear_fallback", "ggufb200_linear_fallback_route",
 )

@@ -131,6 +131,66 @@ static Route pick_route(int type, const void *W, long long M, long long N, long 
     return r;
 }
 
+// ------------------------------------------------------------------ the Linear of the fallback.cuh formats
+// block size and alignment (A_BLK) of a fallback format; false for every other code
+static bool fallback_geom(int t, int *bs, int *a_blk)
+{
+    return with_fallback_block(t, false, [&](auto blk) {
+        if (bs) *bs = decltype(blk)::BS;
+        if (a_blk) *a_blk = decltype(blk)::A_BLK;
+        return true;
+    });
+}
+
+// AUTO: FUSED_SYNC up to this M where the kernel's plan cuts K into ranges (the feature x token tile grid fills at most half the
+// SMs), else DEQUANT_MMA.  Measured on an H100 80GB HBM3 (700 W power limit; tools/bench_linear_fallback.py, the seven
+// Qwen3-4B / Qwen2.5-VL-7B / Mistral-Small-24B shapes, bf16 and fp16, DESIGN.md section 9): the fused kernel is bound by its
+// decoders, not by the packed bytes, so it wins only while it decodes each weight run once (M <= 64, one token tile) and split K
+// puts every SM to work.  Median two-step / fused time on the split shapes at M = 64: 1.03 - 1.13 for the i-quants, 1.03 for
+// TQ2_0, 0.98 / 0.96 for MXFP4 / NVFP4 (1.12 / 1.08 at M = 32); TQ2_0 stops at 32 too (its weakest point at 64: 0.76).  Over the
+// points this rule sends to FUSED_SYNC at 8 < M <= 64 the median is 1.29, the weakest 0.90.  At
+// M = 77 and above: 0.17 - 0.75 for every type.  TQ1_0's decoder (one trit per step) loses at every M (0.69 - 0.77): it stays on
+// DEQUANT_MMA.  Unsplit grids ([9728, 2560] at 76 feature tiles, [18944, 3584], [32768, 5120]) ran at 0.52 - 0.98: DEQUANT_MMA.
+static long long fallback_crossover(int type)
+{
+    switch (type) {
+    case T_TQ1_0: return 0;
+    case T_TQ2_0:
+    case T_MXFP4:
+    case T_NVFP4: return 32;
+    }
+    return 64;
+}
+
+// `W` may be NULL (workspace query: assume an aligned weight)
+static Route pick_fallback_route(int type, const void *W, long long M, long long N, long long K, int algo_flags)
+{
+    int a_blk = 1;
+    fallback_geom(type, nullptr, &a_blk);
+    const bool w_ok = !W || reinterpret_cast<uintptr_t>(W) % a_blk == 0;
+    Route r{algo_flags & GGUFB200_ALGO_MASK, 0};
+    if (!w_ok) r.algo = GGUFB200_ALGO_DEQUANT_MMA;
+    else if (r.algo == GGUFB200_ALGO_AUTO)
+        r.algo = M <= fallback_crossover(type) && fallback_linear_workspace(M, N, K, false) > 0 ? GGUFB200_ALGO_FUSED_SYNC
+                                                                                                : GGUFB200_ALGO_DEQUANT_MMA;
+    if (r.algo == GGUFB200_ALGO_DEQUANT_MMA) r.ws = (size_t)N * (size_t)K * 2;
+    else if (r.algo == GGUFB200_ALGO_FUSED_SYNC) r.ws = fallback_linear_workspace(M, N, K, (algo_flags & GGUFB200_FLAG_NOSPLIT) != 0);
+    return r;
+}
+
+// the argument checks of ggufb200_linear_fallback that need no pointer (0: fine)
+static int fallback_linear_args(int ggml_type, int64_t N, int64_t K, int64_t M, int64_t ldx, int64_t ldy, int act_dtype, int algo)
+{
+    int bs = 0;
+    if (!fallback_geom(ggml_type, &bs, nullptr)) return GGUFB200_E_TYPE;
+    if (act_dtype != kF16 && act_dtype != kBF16) return GGUFB200_E_DTYPE;
+    const int a = algo & GGUFB200_ALGO_MASK;
+    if (a != GGUFB200_ALGO_AUTO && a != GGUFB200_ALGO_FUSED_SYNC && a != GGUFB200_ALGO_DEQUANT_MMA) return GGUFB200_E_UNSUPPORTED;
+    if (algo & ~(GGUFB200_ALGO_MASK | GGUFB200_FLAG_EXACT_W | GGUFB200_FLAG_W_STABLE | GGUFB200_FLAG_NOSPLIT)) return GGUFB200_E_UNSUPPORTED;
+    if (M < 0 || N <= 0 || K <= 0 || K % 8 != 0 || K % bs != 0 || N % 8 != 0 || ldx < K || ldy < N) return GGUFB200_E_SHAPE;
+    return GGUFB200_OK;
+}
+
 extern "C" {
 
 int ggufb200_version(void) { return GGUFB200_VERSION; }
@@ -159,7 +219,8 @@ int ggufb200_type_info(int ggml_type, int *block_size, int *type_size)
 
 int ggufb200_supported(int ggml_type, int op)
 {
-    if (op == GGUFB200_OP_DEQUANT_FALLBACK) return with_fallback_block(ggml_type, 0, [](auto) { return 1; });
+    if (op == GGUFB200_OP_DEQUANT_FALLBACK || op == GGUFB200_OP_LINEAR_FALLBACK || op == GGUFB200_OP_ROWS_FALLBACK)
+        return fallback_geom(ggml_type, nullptr, nullptr) ? 1 : 0;
     if (op == GGUFB200_OP_QUANTIZE) return quantize_supported(ggml_type) ? 1 : 0;
     if (op == GGUFB200_OP_LINEAR_GRAD) return grad_type(ggml_type, nullptr) ? 1 : 0;
     if (!type_geom(ggml_type, nullptr, nullptr)) return 0;
@@ -391,6 +452,61 @@ int ggufb200_dequant_rows(int ggml_type, const void *packed, int64_t n_table_row
     if (int rc = device_check()) return rc;
     return rows_dispatch(ggml_type, packed, n_table_rows, K, (const long long *)rows, n_rows, out, out_dtype, math_dtype,
                          (cudaStream_t)stream);
+}
+
+int ggufb200_dequant_rows_fallback(int ggml_type, const void *packed, int64_t n_table_rows, int64_t K, const int64_t *rows, int64_t n_rows,
+                                   void *out, int out_dtype, void *stream)
+{
+    int bs;
+    if (!fallback_geom(ggml_type, &bs, nullptr)) return GGUFB200_E_TYPE;
+    if (!dtype_ok(out_dtype)) return GGUFB200_E_DTYPE;
+    if (n_rows < 0 || n_table_rows < 0 || K <= 0 || K % bs != 0 || K % 8 != 0) return GGUFB200_E_SHAPE;
+    if (n_rows == 0) return GGUFB200_OK;
+    if (!packed || !rows || !out) return GGUFB200_E_NULL;
+    if (!aligned16(out)) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    return rows_fallback_dispatch(ggml_type, packed, n_table_rows, K, (const long long *)rows, n_rows, out, out_dtype, (cudaStream_t)stream);
+}
+
+size_t ggufb200_linear_fallback_workspace(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int algo)
+{
+    if (fallback_linear_args(ggml_type, N, K, M, K, N, act_dtype, algo) != GGUFB200_OK || M <= 0) return 0;
+    return pick_fallback_route(ggml_type, nullptr, M, N, K, algo).ws;
+}
+
+int ggufb200_linear_fallback_route(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int algo)
+{
+    if (int rc = fallback_linear_args(ggml_type, N, K, M, K, N, act_dtype, algo)) return rc;
+    if (M == 0) return GGUFB200_OK;          // the call returns OK without a route: nothing to compute
+    return pick_fallback_route(ggml_type, nullptr, M, N, K, algo).algo;
+}
+
+int ggufb200_linear_fallback(int ggml_type, const void *W_packed, int64_t N, int64_t K, const void *X, int64_t M, int64_t ldx, int act_dtype,
+                             const void *bias, int bias_dtype, void *Y, int64_t ldy, void *workspace, size_t workspace_bytes, int algo,
+                             void *stream)
+{
+    if (int rc = fallback_linear_args(ggml_type, N, K, M, ldx, ldy, act_dtype, algo)) return rc;
+    if (bias && !dtype_ok(bias_dtype)) return GGUFB200_E_DTYPE;
+    if (M == 0) return GGUFB200_OK;
+    if (!W_packed || !X || !Y) return GGUFB200_E_NULL;
+    if (!aligned16(X) || (ldx % 8) != 0 || !aligned16(Y) || (ldy % 8) != 0) return GGUFB200_E_ALIGN;
+    const size_t ws_avail = (workspace && aligned16(workspace)) ? workspace_bytes : 0;
+    const size_t dense = (size_t)N * (size_t)K * 2;
+    int bs = 1, a_blk = 1;
+    fallback_geom(ggml_type, &bs, &a_blk);
+    // a byte-offset view below the type's block alignment: only the standalone dequant reads it (and needs its workspace)
+    if (reinterpret_cast<uintptr_t>(W_packed) % a_blk != 0 && ws_avail < dense) return GGUFB200_E_ALIGN;
+    const Route r = pick_fallback_route(ggml_type, W_packed, M, N, K, algo);
+    if (workspace && !aligned16(workspace) && r.ws) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (r.algo == GGUFB200_ALGO_FUSED_SYNC)
+        return fallback_linear(ggml_type, W_packed, N, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, workspace, ws_avail,
+                               (algo & GGUFB200_FLAG_NOSPLIT) != 0, st);
+    if (ws_avail < dense) return GGUFB200_E_WORKSPACE;
+    const int rc = fallback_dispatch(ggml_type, W_packed, N * K / bs, workspace, act_dtype, st, (algo & GGUFB200_FLAG_W_STABLE) != 0);
+    if (rc != GGUFB200_OK) return rc;
+    return dense_gemm(workspace, N, K, K, X, M, ldx, act_dtype, bias, bias_dtype, Y, ldy, st);
 }
 
 size_t ggufb200_linear_workspace_ex(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int math_dtype, int algo)

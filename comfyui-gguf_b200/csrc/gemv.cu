@@ -8,6 +8,7 @@
 // (dequant.py:23, ops.py:210) and accumulated in fp32; warp-shuffle reduction at the end.
 #include "blocks.cuh"
 #include "internal.h"
+#include "mma_sync.cuh"
 
 namespace ggufb200 {
 
@@ -22,18 +23,6 @@ template <int ACT> __device__ __forceinline__ float2 act_bits_to_f32x2(uint32_t 
     else return __half22float2(*reinterpret_cast<__half2 *>(&b));
 }
 
-// bias value rounded to the activation dtype first: the reference casts the bias to x.dtype
-// (ops.py:205-207, bias_dtype = dtype) before F.linear adds it
-template <int ACT> __device__ __forceinline__ float load_bias(const void *bias, int bias_dtype, long long n)
-{
-    float b;
-    if (bias_dtype == kF32) b = reinterpret_cast<const float *>(bias)[n];
-    else if (bias_dtype == kF16) b = __half2float(reinterpret_cast<const __half *>(bias)[n]);
-    else b = __bfloat162float(reinterpret_cast<const __nv_bfloat16 *>(bias)[n]);
-    if constexpr (ACT == kBF16) return __bfloat162float(__float2bfloat16_rn(b));
-    else return __half2float(__float2half_rn(b));
-}
-
 // ------------------------------------------------------------------ tensor-core variant (default)
 // The dot products of 16 output features x up to 8 activation rows are one mma.sync.m16n8k16 tile (legacy HMMA path: the
 // kernel is bound by the weight stream, not by flops; a warpgroup MMA needs M = 64 rows and would idle most of them here).
@@ -41,20 +30,7 @@ template <int ACT> __device__ __forceinline__ float load_bias(const void *bias, 
 // permuted freely as long as A and B use the same permutation, so thread (g = lane/4, c = lane%4) simply owns the run of 32
 // consecutive k  [128*span + 32c, +32)  of rows g and g+8 (header decoded once per run) and of activation row g: every
 // 8-element chunk feeds two MMAs, no shuffles, no per-element FMA / unpack.  The 8 warps of a CTA split K and reduce
-// their 16x8 partial tiles through shared memory.
-template <int ACT> __device__ __forceinline__ void mma_16x8x16(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1)
-{
-    if constexpr (ACT == kBF16) {
-        asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                     : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-    } else {
-        asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                     : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-    }
-}
-
+// their 16x8 partial tiles through shared memory.  (mma_16x8x16 and load_bias: mma_sync.cuh.)
 template <class Q, int MATH, int ACT>
 __global__ void __launch_bounds__(kGemvThreads) gemv_mma_kernel(const uint8_t *__restrict__ W, long long N, long long K, const uint8_t *__restrict__ X,
                                                                 long long ldx, int M, const void *__restrict__ bias, int bias_dtype,

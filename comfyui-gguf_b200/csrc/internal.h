@@ -21,6 +21,9 @@ int fallback_dispatch(int type, const void *packed, long long n_blocks, void *ou
 int unpack_dispatch(int type, const void *packed, long long n_blocks, int16_t *q, int16_t *sc, int16_t *mn, cudaStream_t st);
 int rows_dispatch(int type, const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows, void *out,
                   int out_dtype, int math_dtype, cudaStream_t st);
+// ggufb200_dequant_rows_fallback: the row gather for the formats of fallback.cuh (fp32 math); arguments validated by the caller
+int rows_fallback_dispatch(int type, const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows, void *out,
+                           int out_dtype, cudaStream_t st);
 // ggufb200_dequant_kron: the [N, K] weight (whole-block rows or straddled, K % 8 == 0) with LoKr patches applied; `patches` are
 // validated by the caller (api.cu), n_patches <= kKronMaxPatches
 constexpr int kKronMaxPatches = 8;
@@ -109,6 +112,18 @@ void fused_tmem_plan(long long M, long long N, long long K, size_t ws_bytes, con
 int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span_stride, long long N, long long K, const void *X, long long M,
                       long long ldx, int act_dtype, const void *bias, int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes,
                       const LinearOptions &opt, const LoraOperands &lora, cudaStream_t st, const float *scale = nullptr);
+
+// The split-K finalize of the fused routes: Y = act(sum_s P[s] + bias), P fp32 [splits, M, N], slices added in ascending order;
+// N % 8 == 0, Y and ldy as for dense_gemm.
+int split_k_finalize(const float *P, int splits, const void *bias, int bias_dtype, void *Y, long long M, long long N, long long ldy, int act_dtype,
+                     cudaStream_t st);
+
+// ------------------------------------------------------------------ linear_fallback.cu: GGUFB200_ALGO_FUSED_SYNC, the fused Linear of
+// the fallback.cuh formats (arguments validated by the caller: K % 32 == 0, N % 8 == 0, W aligned to the type's A_BLK).
+// `ws_bytes` as above; with too little workspace the kernel uses fewer K ranges, with none it runs unsplit.
+size_t fallback_linear_workspace(long long M, long long N, long long K, bool nosplit);
+int fallback_linear(int type, const void *W, long long N, long long K, const void *X, long long M, long long ldx, int act_dtype, const void *bias,
+                    int bias_dtype, void *Y, long long ldy, void *ws, size_t ws_bytes, bool nosplit, cudaStream_t st);
 
 // ------------------------------------------------------------------ scale.cu: Y = act(fp32(X) * c[k]) (ggufb200_scale_columns)
 int scale_columns_dispatch(const void *X, long long M, long long K, long long ldx, int act_dtype, const float *col_scale, void *Y,

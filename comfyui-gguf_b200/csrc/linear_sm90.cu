@@ -416,4 +416,11 @@ int fused_tmem_linear(int type, const void *W, const void *Wspan, long long span
     });
 }
 
+int split_k_finalize(const float *P, int splits, const void *bias, int bias_dtype, void *Y, long long M, long long N, long long ldy, int act_dtype,
+                     cudaStream_t st)
+{
+    return act_dtype == kBF16 ? wg_finalize<kBF16>(P, splits, bias, bias_dtype, Y, M, N, ldy, st)
+                              : wg_finalize<kF16>(P, splits, bias, bias_dtype, Y, M, N, ldy, st);
+}
+
 }  // namespace ggufb200

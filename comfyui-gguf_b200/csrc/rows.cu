@@ -2,21 +2,25 @@
 //
 // Replaces the Embedding path of the reference (ops.py:251-259), which dequantises the WHOLE
 // table on every call and then runs F.embedding: here only the requested rows are read
-// (K/BS*TS bytes each) and written (K elements each).  One CTA per (row, 2048-element chunk).
+// (K/BS*TS bytes each) and written (K elements each).  One CTA per (row, chunk of 2048 elements; 8192 for the formats of
+// fallback.cuh, whose decoder yields 32 elements per thread).
+// The formats of fallback.cuh go through the same kernel: each thread decodes runs of 32 with Fallback<T>::run32 and rounds the
+// fp32 values once to the output dtype, exactly as ggufb200_dequant_fallback does.
 #include "blocks.cuh"
+#include "fallback.cuh"
 #include "internal.h"
 
 namespace ggufb200 {
 
 constexpr int kRowThreads = 256;
-constexpr int kChunkElems = 2048;
+template <class Q> constexpr int chunk_elems() { return IsFallback<Q>::value ? 8192 : 2048; }
 
 template <class Q, int MATH, int OUT>
 __global__ void __launch_bounds__(kRowThreads) rows_kernel(const uint8_t *__restrict__ table, long long n_table_rows, long long K,
                                                            const long long *__restrict__ rows, void *__restrict__ dst)
 {
-    constexpr int EPT = 16 / OutT<OUT>::bytes;
-    constexpr int CHUNK_BLOCKS = kChunkElems / Q::BS;
+    constexpr int EPT = IsFallback<Q>::value ? 32 : 16 / OutT<OUT>::bytes;
+    constexpr int CHUNK_BLOCKS = chunk_elems<Q>() / Q::BS;
     constexpr int CHUNK_BYTES = CHUNK_BLOCKS * Q::TS;
     __shared__ __align__(16) uint8_t tile[CHUNK_BYTES];
 
@@ -46,16 +50,32 @@ __global__ void __launch_bounds__(kRowThreads) rows_kernel(const uint8_t *__rest
     for (int idx = threadIdx.x * EPT; idx < elems; idx += kRowThreads * EPT) {
         uint8_t *o = o_row + (long long)idx * OutT<OUT>::bytes;
         if (!valid) {  // out-of-range index: defined result (zeros) instead of a device assert
-            st_global_v4(o, 0, 0, 0, 0);
+#pragma unroll
+            for (int j = 0; j < EPT * OutT<OUT>::bytes / 16; ++j) st_global_v4(o + 16 * j, 0, 0, 0, 0);
             continue;
         }
-        typename Math<MATH>::T2 v[EPT / 2];
-        dequant_run<Q, MATH, EPT>(tile + (idx / Q::BS) * Q::TS, idx % Q::BS, v);
-        if constexpr (OUT == kF32) {
-            float2 f0 = Math<MATH>::to_f32x2(v[0]), f1 = Math<MATH>::to_f32x2(v[1]);
-            st_global_v4(o, __float_as_uint(f0.x), __float_as_uint(f0.y), __float_as_uint(f1.x), __float_as_uint(f1.y));
+        if constexpr (IsFallback<Q>::value) {
+            static_assert(MATH == kF32, "the fallback formats are decoded in fp32 only");
+            float f[32];
+            Q::run32(tile + (idx / Q::BS) * Q::TS, idx % Q::BS, f);
+#pragma unroll
+            for (int j = 0; j < 32; j += 16 / OutT<OUT>::bytes) {
+                if constexpr (OUT == kF32) {
+                    st_global_v4(o + 4 * j, __float_as_uint(f[j]), __float_as_uint(f[j + 1]), __float_as_uint(f[j + 2]), __float_as_uint(f[j + 3]));
+                } else {
+                    st_global_v4(o + 2 * j, pack16<OUT, kF32>(make_float2(f[j], f[j + 1])), pack16<OUT, kF32>(make_float2(f[j + 2], f[j + 3])),
+                                 pack16<OUT, kF32>(make_float2(f[j + 4], f[j + 5])), pack16<OUT, kF32>(make_float2(f[j + 6], f[j + 7])));
+                }
+            }
         } else {
-            st_global_v4(o, pack16<OUT, MATH>(v[0]), pack16<OUT, MATH>(v[1]), pack16<OUT, MATH>(v[2]), pack16<OUT, MATH>(v[3]));
+            typename Math<MATH>::T2 v[EPT / 2];
+            dequant_run<Q, MATH, EPT>(tile + (idx / Q::BS) * Q::TS, idx % Q::BS, v);
+            if constexpr (OUT == kF32) {
+                float2 f0 = Math<MATH>::to_f32x2(v[0]), f1 = Math<MATH>::to_f32x2(v[1]);
+                st_global_v4(o, __float_as_uint(f0.x), __float_as_uint(f0.y), __float_as_uint(f1.x), __float_as_uint(f1.y));
+            } else {
+                st_global_v4(o, pack16<OUT, MATH>(v[0]), pack16<OUT, MATH>(v[1]), pack16<OUT, MATH>(v[2]), pack16<OUT, MATH>(v[3]));
+            }
         }
     }
 }
@@ -80,7 +100,7 @@ __global__ void __launch_bounds__(kRowThreads) rows_bf16_kernel(const uint16_t *
 template <class Q, int MATH, int OUT>
 static int launch_rows(const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows, void *out, cudaStream_t st)
 {
-    long long chunks = (K + kChunkElems - 1) / kChunkElems;
+    long long chunks = (K + chunk_elems<Q>() - 1) / chunk_elems<Q>();
     for (long long y0 = 0; y0 < n_rows; y0 += 65535) {  // gridDim.y limit
         long long ny = n_rows - y0 < 65535 ? n_rows - y0 : 65535;
         dim3 grid((unsigned)chunks, (unsigned)ny);
@@ -128,6 +148,14 @@ int rows_dispatch(int type, const void *packed, long long n_table_rows, long lon
     }
     return with_block(type, GGUFB200_E_TYPE, [&](auto blk) {
         return rows_math<decltype(blk)>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, math_dtype, st);
+    });
+}
+
+int rows_fallback_dispatch(int type, const void *packed, long long n_table_rows, long long K, const long long *rows, long long n_rows, void *out,
+                           int out_dtype, cudaStream_t st)
+{
+    return with_fallback_block(type, (int)GGUFB200_E_TYPE, [&](auto blk) {
+        return rows_out<decltype(blk), kF32>(packed, n_table_rows, K, rows, n_rows, out, out_dtype, st);
     });
 }
 

@@ -186,7 +186,9 @@ def unpack_int(data, qtype):
 
 
 def dequantize_rows(tensor, rows, dtype=None, dequant_dtype=None):
-    """out[i] = dequant(W[rows[i]]): the gather the Embedding path needs, without touching other rows."""
+    """out[i] = dequant(W[rows[i]]): the gather the Embedding path needs, without touching other rows.  A FALLBACK_QTYPES
+    table goes through ggufb200_dequant_rows_fallback: dequantize_fallback's values (dtype None = float32, dequant_dtype
+    ignored, as on the reference's `else` branch)."""
     qtype = tensor.tensor_type
     shape = tuple(tensor.tensor_shape)
     n_table, K = shape[0], shape[-1]
@@ -195,6 +197,13 @@ def dequantize_rows(tensor, rows, dtype=None, dequant_dtype=None):
         _require_cuda("dequantize_rows")
         raw = raw.to("cuda")
     rows = rows.to(device=raw.device, dtype=torch.int64).contiguous()
+    if qtype in FALLBACK_QTYPES:
+        out = torch.empty(rows.numel(), K, dtype=torch.float32 if dtype is None else dtype, device=raw.device)
+        with torch.cuda.device(raw.device):
+            rc = _lib.lib().ggufb200_dequant_rows_fallback(int(qtype), raw.data_ptr(), n_table, K, rows.data_ptr(), rows.numel(),
+                                                           out.data_ptr(), dtype_code(out.dtype), _stream_ptr(raw.device))
+        _lib.check(rc, f"ggufb200_dequant_rows_fallback({qtype.name})")
+        return out.reshape(*rows.shape, K)
     out_dtype = torch.float16 if dtype is None else dtype
     if qtype == _Q.BF16 and dtype is None:
         out_dtype = torch.float32

@@ -21,6 +21,7 @@ What changes underneath:
 from __future__ import annotations
 
 import logging
+import math
 
 import gguf
 import torch
@@ -239,6 +240,40 @@ def _launch_linear(x, wraw, qtype, N, K, bias, math, algo, spans=None, lora=None
             rc = call()
     if rc:
         _lib.check(rc, f"ggufb200_linear({getattr(qtype, 'name', qtype)}, M={M}, N={N}, K={K})")
+    return y if x.dim() == 2 else y.reshape(*x.shape[:-1], N)
+
+
+def linear_fallback(x, wraw, qtype, N, K, bias, algo=_lib.ALGO_AUTO | _lib.FLAG_W_STABLE):
+    """y = x @ W.T + bias for a weight in one of FALLBACK_QTYPES (ggufb200_linear_fallback): W is gguf-py's fp32 value rounded
+    once to x.dtype, decoded from the packed rows `wraw` (plain uint8 on x.device) inside the kernel, or dequantised into a
+    workspace above AUTO's crossover M.  x: CUDA fp16/bf16 [..., K]; bias: PLAIN tensor on x.device or None.  W_STABLE: the
+    packed weight is a parameter (or its host-to-device copy), never written by a kernel in flight."""
+    x2 = x if x.dim() == 2 else x.reshape(-1, K)
+    if x2.stride(-1) != 1 or (x2.stride(0) & 7) or (x2.data_ptr() & 15):
+        x2 = x2.contiguous()
+    M = x2.shape[0]
+    device = x.device
+    y = torch.empty((M, N), dtype=x.dtype, device=device)
+    if not wraw.is_contiguous():
+        wraw = wraw.contiguous()
+    bias_ptr, bias_code = None, 0
+    if bias is not None:
+        if not bias.is_contiguous():
+            bias = bias.contiguous()
+        bias_ptr, bias_code = bias.data_ptr(), dtype_code(bias.dtype)
+    L = _lib.lib()
+    qcode, act = int(qtype), dtype_code(x.dtype)
+    # the workspace query assumes a base aligned to the type's blocks (gcd(type_size, 16), fallback.cuh A_BLK); a byte-offset view
+    # below that is read by the standalone dequant only, which the call then takes whatever `algo` says: ask for that route's size
+    query_algo = algo
+    if wraw.data_ptr() % math.gcd(gguf.GGML_QUANT_SIZES[qtype][1], 16):
+        query_algo = _lib.ALGO_DEQUANT_MMA | (algo & ~_lib.ALGO_MASK)
+    need = L.ggufb200_linear_fallback_workspace(qcode, M, N, K, act, query_algo)      # same routing function as the call below
+    ws = torch.empty(need, dtype=torch.uint8, device=device) if need else None
+    with torch.cuda.device(device):
+        rc = L.ggufb200_linear_fallback(qcode, wraw.data_ptr(), N, K, x2.data_ptr(), M, x2.stride(0), act, bias_ptr, bias_code, y.data_ptr(), N,
+                                        None if ws is None else ws.data_ptr(), need, algo, _current_stream_ptr(device.index))
+    _lib.check(rc, f"ggufb200_linear_fallback({getattr(qtype, 'name', qtype)}, M={M}, N={N}, K={K})")
     return y if x.dim() == 2 else y.reshape(*x.shape[:-1], N)
 
 
@@ -1514,9 +1549,21 @@ class GGMLOps(comfy_ops.manual_cast):
                         if N % 8 == 0 and K % 8 == 0:
                             y = self._dora_linear(input, dora, src, wraw, resident, b, M)
                     elif qtype in FALLBACK_QTYPES:
-                        # numpy-fallback types (csrc/fallback.cuh): no fused kernel reads them, so K1 into an [N, K] activation-dtype
-                        # weight (the reference's fp32 -> dtype rounding) + the dense GEMM at every M; other shapes: two-step route
-                        if N % 8 == 0 and K % 8 == 0:
+                        # numpy-fallback types (csrc/fallback.cuh): above M = 8, whole-block rows run on ggufb200_linear_fallback
+                        # where its AUTO decodes the weight from the packed bytes (FUSED_SYNC); everywhere else (AUTO's
+                        # DEQUANT_MMA, M <= 8, rows that straddle blocks) K1 into an [N, K] activation-dtype weight (the
+                        # reference's fp32 -> dtype rounding) + the dense GEMM; other shapes: two-step route.
+                        # Where AUTO would take DEQUANT_MMA the layer keeps issuing the two library calls itself instead of
+                        # one ggufb200_linear_fallback: the work and the bits are the same, and callers that trace the layer
+                        # by the entry points it calls (tests/test_gpu_linear_grad.py::test_no_grad_path_unchanged watches
+                        # ggufb200_dequant_fallback and ggufb200_gemm at M = 300) keep seeing the route they saw before.
+                        # Do not fold this back into one AUTO call.
+                        if (M > GEMV_MAX_M and N % 8 == 0 and K % 8 == 0 and K % gguf.GGML_QUANT_SIZES[qtype][0] == 0
+                                and _lib.lib().ggufb200_linear_fallback_route(int(qtype), M, N, K, dtype_code(input.dtype),
+                                                                              _lib.ALGO_AUTO) == _lib.ALGO_FUSED_SYNC):
+                            def run():
+                                return linear_fallback(input, wraw, qtype, N, K, b)
+                        elif N % 8 == 0 and K % 8 == 0:
                             def run():
                                 return linear_dense(input, dequantize_fallback(wraw, qtype, (N, K), input.dtype), b)
                     elif kron is not None:
@@ -1687,8 +1734,10 @@ class GGMLOps(comfy_ops.manual_cast):
             if self.weight.dtype in (torch.float16, torch.bfloat16):
                 out_dtype = None
             w = self.weight
-            plain_case = (self.max_norm is None and not getattr(w, "patches", None) and input.is_cuda
-                          and len(getattr(w, "tensor_shape", ())) == 2 and getattr(w, "tensor_type", None) not in FALLBACK_QTYPES)
+            qtype = getattr(w, "tensor_type", None)
+            shape = tuple(getattr(w, "tensor_shape", ()))
+            plain_case = (self.max_norm is None and not getattr(w, "patches", None) and input.is_cuda and len(shape) == 2
+                          and (qtype not in FALLBACK_QTYPES or (shape[1] % 8 == 0 and shape[1] % gguf.GGML_QUANT_SIZES[qtype][0] == 0)))
             if plain_case:
                 w = w if w.device == input.device else w.to(input.device)
                 # the reference passes the module itself as `input` to cast_bias_weight (ops.py:256), so a missing

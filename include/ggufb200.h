@@ -59,6 +59,8 @@ extern "C" {
 #define GGUFB200_OP_DEQUANT_FALLBACK 4 /* ggufb200_dequant_fallback() serves this type */
 #define GGUFB200_OP_QUANTIZE 5 /* ggufb200_quantize() produces this type */
 #define GGUFB200_OP_LINEAR_GRAD 6 /* ggufb200_linear_grad_input() serves this type */
+#define GGUFB200_OP_LINEAR_FALLBACK 7 /* ggufb200_linear_fallback() serves this type */
+#define GGUFB200_OP_ROWS_FALLBACK 8 /* ggufb200_dequant_rows_fallback() serves this type */
 
 /* algorithm selector for ggufb200_linear(): one GGUFB200_ALGO_* value, optionally OR-ed with GGUFB200_FLAG_* bits */
 #define GGUFB200_ALGO_AUTO 0
@@ -68,6 +70,7 @@ extern "C" {
 #define GGUFB200_ALGO_FUSED_TMEM 4  /* fused dequant -> shared memory -> wgmma with token tiles sized to M, any M (what AUTO picks for M > 8) */
 #define GGUFB200_ALGO_GEMV_FAST 5   /* M <= 8, Q4_K / Q5_K: integer patterns on mma.sync, sub-block scales applied to the partial sums
                                        (W is never formed or rounded: the `fast` contract; AUTO picks it only without EXACT_W) */
+#define GGUFB200_ALGO_FUSED_SYNC 6  /* ggufb200_linear_fallback only: the weight decoded in registers, mma.sync over up to 64 tokens */
 #define GGUFB200_ALGO_MASK 0xFF
 
 /* Per-call switches (no process-wide state):
@@ -140,7 +143,8 @@ int ggufb200_dequant(int ggml_type, const void *packed, int64_t n_blocks, void *
  *   flags      0 or GGUFB200_DEQUANT_SRC_STABLE (as in ggufb200_dequant); any other bit: GGUFB200_E_UNSUPPORTED
  * Any other ggml_type, including the types of ggufb200_dequant, returns GGUFB200_E_TYPE; ggufb200_supported(t,
  * GGUFB200_OP_DEQUANT_FALLBACK) lists exactly these eleven.  ggufb200_type_info, GGUFB200_OP_DEQUANT, the Linear entry points
- * and ggufb200_dequant_rows keep the reference's table (dequant.py:287-301) only.
+ * and ggufb200_dequant_rows keep the reference's table (dequant.py:287-301) only; these types have their own Linear
+ * (ggufb200_linear_fallback) and row gather (ggufb200_dequant_rows_fallback).
  */
 int ggufb200_dequant_fallback(int ggml_type, const void *packed, int64_t n_blocks, void *out, int out_dtype, int flags,
                               void *stream);
@@ -294,6 +298,18 @@ int ggufb200_dequant_rows(int ggml_type, const void *packed, int64_t n_table_row
                           void *stream);
 
 /*
+ * Row gather of the types of ggufb200_dequant_fallback: out[i, :] = dequant(W[rows[i], :]), every element bit-identical to
+ * ggufb200_dequant_fallback's value for that row (gguf-py's fp32 value rounded once to out_dtype; no math dtype).  Replaces, for
+ * an Embedding table in one of these types, the reference's dequantisation of the whole table on every call.
+ *   packed     n_table_rows rows of K / block_size * type_size bytes, any alignment; K % block_size == 0 and K % 8 == 0
+ *   rows       n_rows int64 indices on the device; an index outside 0 .. n_table_rows - 1 gives a row of zeros
+ *   out        n_rows * K elements of out_dtype (0 / 1 / 2), 16-byte aligned
+ * Any other ggml_type: GGUFB200_E_TYPE (ggufb200_supported(t, GGUFB200_OP_ROWS_FALLBACK) lists exactly the eleven types).
+ */
+int ggufb200_dequant_rows_fallback(int ggml_type, const void *packed, int64_t n_table_rows, int64_t K, const int64_t *rows, int64_t n_rows,
+                                   void *out, int out_dtype, void *stream);
+
+/*
  * Fused Linear: Y[M,N] = X[M,K] * dequant(W)[N,K]^T (+ bias[N]).  Replaces
  * ops.py:242-244 `forward_ggml_cast_weights` = cast_bias_weight (ops.py:193-211)
  * -> get_weight/dequantize_tensor (ops.py:166-191) -> F.linear.
@@ -328,6 +344,39 @@ size_t ggufb200_linear_workspace_ex(int ggml_type, int64_t M, int64_t N, int64_t
 int ggufb200_linear(int ggml_type, const void *W_packed, int64_t N, int64_t K, const void *X, int64_t M,
                     int64_t ldx, int act_dtype, int math_dtype, const void *bias, int bias_dtype, void *Y,
                     int64_t ldy, void *workspace, size_t workspace_bytes, int algo, void *stream);
+
+/*
+ * Linear on a weight in one of the types of ggufb200_dequant_fallback: Y[M,N] = X[M,K] * W[N,K]^T (+ bias[N]), W = gguf-py's fp32
+ * values rounded once to act_dtype (bit-identical to ggufb200_dequant_fallback's output), fp32 accumulation, the bias rounded to
+ * act_dtype first.  Replaces, for these types, the reference's numpy dequantisation + F.linear.  There is one contract, so there
+ * is no math dtype and GGUFB200_FLAG_EXACT_W is accepted with no effect.
+ *   W_packed   N rows of K / block_size * type_size bytes; K % block_size == 0, K % 8 == 0, N % 8 == 0 (GGUFB200_E_SHAPE)
+ *   X, Y       act_dtype (0 fp16 / 1 bf16), row strides ldx >= K and ldy >= N in ELEMENTS, multiples of 8, 16-byte aligned
+ *   bias       NULL or N values of bias_dtype (0/1/2)
+ *   workspace  at least ggufb200_linear_fallback_workspace() bytes, 16-byte aligned (may be NULL if that is 0)
+ *   algo       GGUFB200_ALGO_FUSED_SYNC: the weight decoded in registers from the packed bytes, never written to memory.  With
+ *                  few feature x token tiles K is cut into ranges whose fp32 partial results go to the workspace and are summed
+ *                  in a fixed order (reproducible); with less workspace it uses fewer ranges, with none it runs unsplit.
+ *              GGUFB200_ALGO_DEQUANT_MMA: ggufb200_dequant_fallback into the workspace (N * K * 2 bytes), then the dense GEMM.
+ *              GGUFB200_ALGO_AUTO: FUSED_SYNC up to a per-type crossover M where FUSED_SYNC would cut K into ranges,
+ *                  DEQUANT_MMA otherwise (DESIGN.md section 9).
+ *              GEMV, GEMV_FAST, FUSED_MMA, FUSED_TMEM: GGUFB200_E_UNSUPPORTED.
+ *              Flags: GGUFB200_FLAG_W_STABLE (passed on to the dequant of DEQUANT_MMA as GGUFB200_DEQUANT_SRC_STABLE),
+ *              GGUFB200_FLAG_EXACT_W (no effect), GGUFB200_FLAG_NOSPLIT (FUSED_SYNC never cuts K); any other bit:
+ *              GGUFB200_E_UNSUPPORTED.
+ * A W_packed that is not aligned to its type's block alignment (gcd(type_size, 16): a byte-offset view) is always served by
+ * GGUFB200_ALGO_DEQUANT_MMA, which reads any alignment, and needs that algo's workspace (GGUFB200_E_ALIGN without it).
+ * ggufb200_linear_fallback_workspace() returns the workspace of the route the call takes for an aligned weight (query and call
+ * always agree), 0 for arguments the call refuses.  ggufb200_linear_fallback_route() returns that route
+ * (GGUFB200_ALGO_FUSED_SYNC or GGUFB200_ALGO_DEQUANT_MMA), GGUFB200_OK for M == 0 (the call computes nothing), or the error
+ * code the call would return for these arguments; the packed Linear layer runs the two steps of DEQUANT_MMA itself when AUTO
+ * would take them.
+ */
+size_t ggufb200_linear_fallback_workspace(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int algo);
+int ggufb200_linear_fallback_route(int ggml_type, int64_t M, int64_t N, int64_t K, int act_dtype, int algo);
+int ggufb200_linear_fallback(int ggml_type, const void *W_packed, int64_t N, int64_t K, const void *X, int64_t M, int64_t ldx, int act_dtype,
+                             const void *bias, int bias_dtype, void *Y, int64_t ldy, void *workspace, size_t workspace_bytes, int algo,
+                             void *stream);
 
 /*
  * Span-major shadow layout (SURVEY 8f rank 3, "one-time GPU repack").  The canonical GGUF rows (loader.py:96-120) can be
