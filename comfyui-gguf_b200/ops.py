@@ -1736,8 +1736,10 @@ class GGMLOps(comfy_ops.manual_cast):
             w = self.weight
             qtype = getattr(w, "tensor_type", None)
             shape = tuple(getattr(w, "tensor_shape", ()))
+            # the row gather needs whole blocks and K % 8 == 0 for every type (a BF16 table can be any width); any other table
+            # takes the whole-table dequant below
             plain_case = (self.max_norm is None and not getattr(w, "patches", None) and input.is_cuda and len(shape) == 2
-                          and (qtype not in FALLBACK_QTYPES or (shape[1] % 8 == 0 and shape[1] % gguf.GGML_QUANT_SIZES[qtype][0] == 0)))
+                          and shape[1] % 8 == 0 and shape[1] % gguf.GGML_QUANT_SIZES[qtype][0] == 0)
             if plain_case:
                 w = w if w.device == input.device else w.to(input.device)
                 # the reference passes the module itself as `input` to cast_bias_weight (ops.py:256), so a missing
