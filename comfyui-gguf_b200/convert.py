@@ -17,6 +17,11 @@ convert_file() writes in one pass what the reference's two steps write:
       the Q types, its rows are a multiple of 32 long (F16 / BF16 take any row); ffn_down-type tensors go from Q4_0 to Q4_1 and from
       Q5_0 to Q5_1.  The quantiser reads the value the stage-1 file holds (fp32 rounded to fp16, bf16 exact), so the bytes
       are those of the two-step pipeline.  Quantisation runs on the GPU (quantize.py); tensors come back one at a time.
+  K mixtures (`qtype` one of KQUANT_MIXTURES' names: Q2_K, Q3_K_S / M / L, Q4_K_S / M, Q5_K_S / M, Q6_K, llama-quantize's file
+      types): the same tensors are quantised, each to the type the patch's img_tensor_get_type picks: the mixture's default
+      K type, raised for attention-value, fused-qkv and ffn_down tensors as the table says (the attention-value rule of Q3_K_M
+      and Q4_K_S depends on how many attention-value tensors came before, in file order); a tensor whose rows are not a
+      multiple of 256 then becomes F16, even when stage 1 holds BF16.  The K bytes come from quantize_k_tensor.
 Tensors are written in input order with their full shapes.
 """
 from __future__ import annotations
@@ -154,6 +159,43 @@ _FFN_DOWN = ("ffn_down", ".ffn.2.weight", ".ff.net.2.weight", ".mlp.layer2.weigh
 _FFN_UPGRADE = {_Q.Q4_0: _Q.Q4_1, _Q.Q5_0: _Q.Q5_1}
 
 
+# llama-quantize's K mixtures (the patch's img_tensor_get_type): default type, general.file_type, and the raised types of the
+# attention-value tensors ((n, type) pairs: the i-th attention-value tensor gets the type of the first pair with i < n, else the
+# default), of the fused-qkv tensors and of the ffn_down tensors (None: the default)
+@dataclass(frozen=True)
+class KMixture:
+    name: str
+    default: _Q
+    file_type: gguf.LlamaFileType
+    attn_v: tuple = ()
+    qkv: _Q | None = None
+    ffn_down: _Q | None = None
+
+
+_ALL = 1 << 62
+_FT = gguf.LlamaFileType
+KQUANT_MIXTURES = {m.name: m for m in (
+    KMixture("Q2_K", _Q.Q2_K, _FT.MOSTLY_Q2_K, attn_v=((_ALL, _Q.Q3_K),)),
+    KMixture("Q3_K_S", _Q.Q3_K, _FT.MOSTLY_Q3_K_S),
+    KMixture("Q3_K_M", _Q.Q3_K, _FT.MOSTLY_Q3_K_M, attn_v=((2, _Q.Q5_K), (_ALL, _Q.Q4_K)), qkv=_Q.Q4_K, ffn_down=_Q.Q4_K),
+    KMixture("Q3_K_L", _Q.Q3_K, _FT.MOSTLY_Q3_K_L, attn_v=((_ALL, _Q.Q5_K),), qkv=_Q.Q4_K, ffn_down=_Q.Q5_K),
+    KMixture("Q4_K_S", _Q.Q4_K, _FT.MOSTLY_Q4_K_S, attn_v=((4, _Q.Q5_K),), ffn_down=_Q.Q5_K),
+    KMixture("Q4_K_M", _Q.Q4_K, _FT.MOSTLY_Q4_K_M, attn_v=((_ALL, _Q.Q6_K),), qkv=_Q.Q5_K, ffn_down=_Q.Q6_K),
+    KMixture("Q5_K_S", _Q.Q5_K, _FT.MOSTLY_Q5_K_S),
+    KMixture("Q5_K_M", _Q.Q5_K, _FT.MOSTLY_Q5_K_M, attn_v=((_ALL, _Q.Q6_K),), qkv=_Q.Q6_K, ffn_down=_Q.Q6_K),
+    KMixture("Q6_K", _Q.Q6_K, _FT.MOSTLY_Q6_K),
+)}
+KQUANT_TYPES = (_Q.Q2_K, _Q.Q3_K, _Q.Q4_K, _Q.Q5_K, _Q.Q6_K)
+
+
+def is_attn_v(name: str) -> bool:
+    return any(p in name for p in _ATTN_V)
+
+
+def is_attn_qkv(name: str) -> bool:
+    return not is_attn_v(name) and any(p in name for p in _ATTN_QKV)
+
+
 def is_ffn_down(name: str) -> bool:
     if any(p in name for p in _ATTN_V + _ATTN_QKV):
         return False
@@ -184,20 +226,37 @@ def ggml_n_dims(shape) -> int:
     return max(len(shape) - lead, 1)
 
 
+def quantisable(key: str, stage1: _Q, stored_shape, arch: Arch) -> bool:
+    """Whether llama-quantize with the image-model patch quantises `key` at all (the row-length check aside)."""
+    if stage1 not in (_Q.F16, _Q.BF16) or ggml_n_dims(stored_shape) != 2:
+        return False
+    if not key.endswith("weight") or "_norm.weight" in key:
+        return False
+    return not (any(k in key for k in arch.keep) or key in arch.keep_names)
+
+
 def stage2_type(key: str, stage1: _Q, stored_shape, arch: Arch, qtype) -> _Q:
     """The type `key` is written in when the file is quantised to `qtype` (None: stage 1 only).  `stored_shape` is the shape
     stage 1 writes (after the SD1 / SDXL reshape)."""
-    if qtype is None or stage1 not in (_Q.F16, _Q.BF16) or ggml_n_dims(stored_shape) != 2:
-        return stage1
-    if not key.endswith("weight") or "_norm.weight" in key:
-        return stage1
-    if any(k in key for k in arch.keep) or key in arch.keep_names:
+    if qtype is None or not quantisable(key, stage1, stored_shape, arch):
         return stage1
     if qtype not in (_Q.F16, _Q.BF16) and stored_shape[-1] % 32 != 0:     # F16 / BF16 have 1-element blocks
         return stage1
     if qtype in _FFN_UPGRADE and is_ffn_down(key):
         return _FFN_UPGRADE[qtype]
     return qtype
+
+
+def kquant_type(key: str, stored_shape, mix: KMixture, n_attn_v: int) -> _Q:
+    """The type of a quantisable tensor in K mixture `mix`, `n_attn_v` attention-value tensors having come before it."""
+    qtype = mix.default
+    if is_attn_v(key):
+        qtype = next((t for n, t in mix.attn_v if n_attn_v < n), mix.default)
+    elif is_attn_qkv(key):
+        qtype = mix.qkv or mix.default
+    elif is_ffn_down(key):
+        qtype = mix.ffn_down or mix.default
+    return qtype if stored_shape[-1] % 256 == 0 else _Q.F16
 
 
 @dataclass
@@ -210,8 +269,9 @@ class TensorPlan:
 
 
 def plan_tensors(state_dict: dict, arch: Arch, qtype=None) -> list:
-    """Every written tensor's plan, in input order; ignored keys are left out."""
+    """Every written tensor's plan, in input order; ignored keys are left out.  `qtype`: None, a type, or a KMixture."""
     plans = []
+    n_attn_v = 0
     for key, t in state_dict.items():
         if any(x in key for x in arch.ignore):
             logging.info(f"Filtering ignored key: '{key}'")
@@ -221,7 +281,14 @@ def plan_tensors(state_dict: dict, arch: Arch, qtype=None) -> list:
         orig = None
         if reshape:
             orig, shape = shape, (t.numel() // 256, 256)
-        plans.append(TensorPlan(key, shape, orig, stage1, stage2_type(key, stage1, shape, arch, qtype)))
+        if isinstance(qtype, KMixture):
+            final = stage1
+            if quantisable(key, stage1, shape, arch):
+                final = kquant_type(key, shape, qtype, n_attn_v)
+                n_attn_v += is_attn_v(key)        # counted before the row check, as the patch does
+        else:
+            final = stage2_type(key, stage1, shape, arch, qtype)
+        plans.append(TensorPlan(key, shape, orig, stage1, final))
     return plans
 
 
@@ -259,10 +326,11 @@ def tensor_bytes(t: torch.Tensor, plan: TensorPlan, device=None) -> np.ndarray:
     v = _stage1_values(t, plan.stage1).reshape(plan.shape)
     if not needs_quantiser(plan):
         return _host_bytes(v, plan.qtype).reshape(-1)
-    from .quantize import quantize_tensor
+    from .quantize import quantize_k_tensor, quantize_tensor
     if device is None:
         device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-    packed = quantize_tensor(v.to(device, non_blocking=False), plan.qtype)
+    encode = quantize_k_tensor if plan.qtype in KQUANT_TYPES else quantize_tensor
+    packed = encode(v.to(device, non_blocking=False), plan.qtype)
     return packed.cpu().numpy().reshape(-1)
 
 
@@ -276,12 +344,15 @@ class ConvertResult:
 
 def convert_state_dict(state_dict: dict, dst_path: str, qtype=None, arch: Arch | None = None, device=None) -> ConvertResult:
     """Write the GGUF file of a prefix-stripped state dict (see the module docstring).  `qtype`: None (the F16 / BF16 file),
-    one of QTYPES' names or values."""
+    one of QTYPES' names or values, or one of KQUANT_MIXTURES' names (or a KMixture)."""
     if isinstance(qtype, str):
-        if qtype.upper() not in QTYPES:
-            raise ValueError(f"unsupported qtype {qtype!r}: one of {', '.join(QTYPES)}")
-        qtype = QTYPES[qtype.upper()]
-    elif qtype is not None:
+        if qtype.upper() in KQUANT_MIXTURES:
+            qtype = KQUANT_MIXTURES[qtype.upper()]
+        elif qtype.upper() not in QTYPES:
+            raise ValueError(f"unsupported qtype {qtype!r}: one of {', '.join(list(QTYPES) + list(KQUANT_MIXTURES))}")
+        else:
+            qtype = QTYPES[qtype.upper()]
+    elif qtype is not None and not isinstance(qtype, KMixture):
         qtype = _Q(qtype)
         if qtype not in FILE_TYPES:
             raise ValueError(f"unsupported qtype {qtype.name}: one of {', '.join(QTYPES)}")
@@ -294,6 +365,8 @@ def convert_state_dict(state_dict: dict, dst_path: str, qtype=None, arch: Arch |
         dtypes = [t.dtype for t in state_dict.values()]
         main = max(set(dtypes), key=dtypes.count) if dtypes else torch.float16
         file_type = gguf.LlamaFileType.MOSTLY_BF16 if main == torch.bfloat16 else gguf.LlamaFileType.MOSTLY_F16
+    elif isinstance(qtype, KMixture):
+        file_type = qtype.file_type
     else:
         file_type = FILE_TYPES[qtype]
     plans = plan_tensors(state_dict, arch, qtype)
@@ -334,7 +407,7 @@ def convert_file(src_path: str, dst_path: str | None = None, qtype=None, overwri
     arch = detect_arch(sd.keys())
     logging.info(f"* Architecture detected from input: {arch.name}")
     if qtype is not None:
-        name = qtype.upper() if isinstance(qtype, str) else _Q(qtype).name
+        name = qtype.upper() if isinstance(qtype, str) else qtype.name if isinstance(qtype, KMixture) else _Q(qtype).name
     else:
         dtypes = [t.dtype for t in sd.values()]
         name = "BF16" if dtypes and max(set(dtypes), key=dtypes.count) == torch.bfloat16 else "F16"

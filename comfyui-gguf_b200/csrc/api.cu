@@ -222,6 +222,7 @@ int ggufb200_supported(int ggml_type, int op)
     if (op == GGUFB200_OP_DEQUANT_FALLBACK || op == GGUFB200_OP_LINEAR_FALLBACK || op == GGUFB200_OP_ROWS_FALLBACK)
         return fallback_geom(ggml_type, nullptr, nullptr) ? 1 : 0;
     if (op == GGUFB200_OP_QUANTIZE) return quantize_supported(ggml_type) ? 1 : 0;
+    if (op == GGUFB200_OP_QUANTIZE_K) return quantize_k_supported(ggml_type) ? 1 : 0;
     if (op == GGUFB200_OP_LINEAR_GRAD) return grad_type(ggml_type, nullptr) ? 1 : 0;
     if (!type_geom(ggml_type, nullptr, nullptr)) return 0;
     switch (op) {
@@ -289,6 +290,19 @@ int ggufb200_quantize(int ggml_type, const void *src, int src_dtype, int64_t n_b
     if (reinterpret_cast<uintptr_t>(src) % (src_dtype == GGUFB200_F32 ? 4 : 2) != 0) return GGUFB200_E_ALIGN;
     if (int rc = device_check()) return rc;
     return quantize_dispatch(ggml_type, src, src_dtype, n_blocks, packed, (cudaStream_t)stream);
+}
+
+int ggufb200_quantize_k(int ggml_type, const void *src, int src_dtype, int64_t n_blocks, void *packed, int flags, void *stream)
+{
+    if (!quantize_k_supported(ggml_type)) return GGUFB200_E_TYPE;
+    if (flags != 0) return GGUFB200_E_UNSUPPORTED;
+    if (!dtype_ok(src_dtype)) return GGUFB200_E_DTYPE;
+    if (n_blocks < 0) return GGUFB200_E_SHAPE;
+    if (n_blocks == 0) return GGUFB200_OK;
+    if (!src || !packed) return GGUFB200_E_NULL;
+    if (reinterpret_cast<uintptr_t>(src) % (src_dtype == GGUFB200_F32 ? 4 : 2) != 0) return GGUFB200_E_ALIGN;
+    if (int rc = device_check()) return rc;
+    return quantize_k_dispatch(ggml_type, src, src_dtype, n_blocks, packed, (cudaStream_t)stream);
 }
 
 int ggufb200_dequant_kron(int ggml_type, const void *packed, int64_t N, int64_t K, void *out, int out_dtype, int math_dtype,

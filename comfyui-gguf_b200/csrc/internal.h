@@ -46,6 +46,9 @@ int dequant_patched_dispatch(int type, const void *packed, long long N, long lon
 // the caller (api.cu)
 bool quantize_supported(int type);
 int quantize_dispatch(int type, const void *src, int src_dtype, long long n_blocks, void *packed, cudaStream_t st);
+// quantize.cu, ggufb200_quantize_k: dense fp32 / fp16 / bf16 -> packed Q2_K / Q3_K / Q4_K / Q5_K / Q6_K (n_blocks super-blocks)
+bool quantize_k_supported(int type);
+int quantize_k_dispatch(int type, const void *src, int src_dtype, long long n_blocks, void *packed, cudaStream_t st);
 
 // ------------------------------------------------------------------ small-M Linear: gemv.cu (GGUFB200_ALGO_GEMV), gemv2.cu (GEMV_FAST)
 int gemv_max_m();

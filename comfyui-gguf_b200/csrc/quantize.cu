@@ -7,7 +7,9 @@
 //     bank conflicts).  Each thread then quantises one block (quantize.cuh) into the packed output tile in shared memory, and the
 //     CTA writes that tile out with consecutive 16-byte stores: every global access of a warp covers whole contiguous lines.
 //   * BF16: elementwise, 8 elements per thread with 16-byte loads and stores when both pointers allow them.
-// Both kernels are launched with programmatic stream serialization, like K1: they wait for the preceding kernel
+//   * K types (ggufb200_quantize_k, Q2_K ... Q6_K): the same staging and stores around a per-group search (quantize_k_kernel
+//     below).  Not bound by HBM: the searches run hundreds of separately rounded fp32 operations per element.
+// All kernels are launched with programmatic stream serialization, like K1: they wait for the preceding kernel
 // (griddepcontrol.wait) before their first global access, and let the next kernel launch (griddepcontrol.launch_dependents)
 // only after their last global store, fenced and joined across the CTA (publish_and_release).  A consumer that promises a
 // stable source (GGUFB200_DEQUANT_SRC_STABLE, GGUFB200_FLAG_W_STABLE) may read the packed bytes before its own wait, so the
@@ -130,6 +132,84 @@ template <int SRC> __global__ void __launch_bounds__(kB16Threads) bf16_quantize_
     publish_and_release();
 }
 
+// K types: one thread per group of 16 (Q2_K, Q3_K, Q6_K) or 32 (Q4_K, Q5_K) values, so a CTA of 128 threads holds 8 or 16
+// super-blocks.  The source tile is staged like the legacy kernel's, one group per padded row.  Each thread runs its group's
+// serial search (the sums must stay in the reference's order, so they are not split across lanes); one thread per super-block
+// then writes the header (scales, mins, d, dmin); each thread recomputes its group's codes from the quantised header into a
+// shared code tile; the CTA packs the code bytes into the output tile and writes it with 16-byte stores.
+constexpr int kKThreads = 128;
+
+template <class KQ, int SRC>
+__global__ void __launch_bounds__(kKThreads) quantize_k_kernel(const void *__restrict__ src, long long n_blocks, uint8_t *__restrict__ dst,
+                                                               int flags)
+{
+    constexpr int GS = KQ::GS, NG = KQ::NG, SB = kKThreads / NG, ROW = GS + 1;
+    constexpr int EB = SRC == kF32 ? 4 : 2;
+    constexpr int VE = 16 / EB;                          // divides GS: a vector stays inside one group's row
+    constexpr int TILE_BYTES = SB * KQ::TS;              // a multiple of 16 for every K type
+    static_assert(TILE_BYTES % 16 == 0 && GS % VE == 0, "tile geometry");
+    __shared__ float stage[kKThreads * ROW];
+    __shared__ KFit fits[kKThreads];
+    __shared__ uint8_t codes[SB * 256];
+    __shared__ bool zero[SB];
+    __shared__ __align__(16) uint8_t otile[TILE_BYTES];
+
+    const int tid = threadIdx.x;
+    const long long b0 = (long long)blockIdx.x * SB;
+    const int nb = n_blocks - b0 < SB ? (int)(n_blocks - b0) : SB;
+    const int n = nb * 256;
+    const long long e0 = b0 * 256;
+
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    if (flags & 1) {
+        const uint4 *s = reinterpret_cast<const uint4 *>(reinterpret_cast<const uint8_t *>(src) + e0 * EB);
+        for (int v = tid; v < n / VE; v += kKThreads) {
+            float f[VE];
+            widen16<SRC>(__ldg(s + v), f);
+            const int e = v * VE;
+            float *row = stage + (e / GS) * ROW + (e % GS);
+#pragma unroll
+            for (int j = 0; j < VE; ++j) row[j] = f[j];
+        }
+    } else {
+        for (int e = tid; e < n; e += kKThreads) stage[(e / GS) * ROW + (e % GS)] = widen<SRC>(src, e0 + e);
+    }
+    __syncthreads();
+    const int sb = tid / NG, j = tid % NG;
+    const bool live = sb < nb;
+    const float *x = stage + tid * ROW;
+    uint8_t *L = codes + sb * 256 + j * GS;
+    if (live) fits[tid] = KQ::fit(x, L);
+    __syncthreads();
+    if (live && j == 0) zero[sb] = KQ::header(fits + sb * NG, otile + sb * KQ::TS);
+    __syncthreads();
+    if (live) {
+        float d, dm;
+        KQ::group_scale(otile + sb * KQ::TS, j, d, dm);
+        if (zero[sb]) {
+            for (int i = 0; i < GS; ++i) L[i] = 0;
+        } else if (d != 0.0f) {
+            KQ::codes(x, d, dm, L);
+        }
+    }
+    __syncthreads();
+    for (int i = tid; i < nb * KQ::PB; i += kKThreads) {
+        const int s = i / KQ::PB, b = i % KQ::PB;
+        otile[s * KQ::TS + KQ::PO + b] = KQ::code_byte(codes + s * 256, b);
+    }
+    __syncthreads();
+    const int bytes = nb * KQ::TS;
+    uint8_t *out = dst + b0 * KQ::TS;
+    int done = 0;
+    if (flags & 2) {
+        done = bytes & ~15;
+        for (int i = tid; i < done / 16; i += kKThreads)
+            reinterpret_cast<uint4 *>(out)[i] = reinterpret_cast<const uint4 *>(otile)[i];
+    }
+    for (int i = done + tid; i < bytes; i += kKThreads) out[i] = otile[i];
+    publish_and_release();
+}
+
 template <class Kernel, class... Args> int launch_pdl(Kernel kern, long long grid, int threads, cudaStream_t st, Args... args)
 {
     if (grid > 0x7fffffffll) return GGUFB200_E_SHAPE;
@@ -163,6 +243,17 @@ template <int SRC> int quantize_src(int type, const void *src, long long n_block
     });
 }
 
+template <int SRC> int quantize_k_src(int type, const void *src, long long n_blocks, void *packed, cudaStream_t st)
+{
+    const int flags = (aligned16(src) ? 1 : 0) | (aligned16(packed) ? 2 : 0);
+    return with_kquant_block(type, (int)GGUFB200_E_TYPE, [&](auto blk) {
+        using KQ = decltype(blk);
+        constexpr int SB = kKThreads / KQ::NG;
+        const long long grid = (n_blocks + SB - 1) / SB;
+        return launch_pdl(quantize_k_kernel<KQ, SRC>, grid, kKThreads, st, src, n_blocks, reinterpret_cast<uint8_t *>(packed), flags);
+    });
+}
+
 }  // namespace
 
 bool quantize_supported(int type) { return type == T_BF16 || with_quant_block(type, false, [](auto) { return true; }); }
@@ -174,6 +265,19 @@ int quantize_dispatch(int type, const void *src, int src_dtype, long long n_bloc
     case kF32: return quantize_src<kF32>(type, src, n_blocks, packed, st);
     case kF16: return quantize_src<kF16>(type, src, n_blocks, packed, st);
     case kBF16: return quantize_src<kBF16>(type, src, n_blocks, packed, st);
+    }
+    return GGUFB200_E_DTYPE;
+}
+
+bool quantize_k_supported(int type) { return with_kquant_block(type, false, [](auto) { return true; }); }
+
+int quantize_k_dispatch(int type, const void *src, int src_dtype, long long n_blocks, void *packed, cudaStream_t st)
+{
+    if (n_blocks == 0) return GGUFB200_OK;
+    switch (src_dtype) {
+    case kF32: return quantize_k_src<kF32>(type, src, n_blocks, packed, st);
+    case kF16: return quantize_k_src<kF16>(type, src, n_blocks, packed, st);
+    case kBF16: return quantize_k_src<kBF16>(type, src, n_blocks, packed, st);
     }
     return GGUFB200_E_DTYPE;
 }

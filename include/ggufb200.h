@@ -61,6 +61,7 @@ extern "C" {
 #define GGUFB200_OP_LINEAR_GRAD 6 /* ggufb200_linear_grad_input() serves this type */
 #define GGUFB200_OP_LINEAR_FALLBACK 7 /* ggufb200_linear_fallback() serves this type */
 #define GGUFB200_OP_ROWS_FALLBACK 8 /* ggufb200_dequant_rows_fallback() serves this type */
+#define GGUFB200_OP_QUANTIZE_K 9 /* ggufb200_quantize_k() produces this type */
 
 /* algorithm selector for ggufb200_linear(): one GGUFB200_ALGO_* value, optionally OR-ed with GGUFB200_FLAG_* bits */
 #define GGUFB200_ALGO_AUTO 0
@@ -278,6 +279,25 @@ int ggufb200_dequant_patched_dora(int ggml_type, const void *packed, int64_t N, 
  *   stream     a cudaStream_t, as everywhere in this header
  */
 int ggufb200_quantize(int ggml_type, const void *src, int src_dtype, int64_t n_blocks, void *packed, int flags, void *stream);
+
+/*
+ * Quantise dense values into packed K-quant super-blocks: Q2_K=10 Q3_K=11 Q4_K=12 Q5_K=13 Q6_K=14, 256 values per super-block.
+ * The encoders restate llama.cpp's reference quantisers at tag b3962 without an importance matrix (what `llama-quantize` runs
+ * without --imatrix): quantize_row_q{2,3,4,5,6}_K_ref with make_qkx2_quants, make_q3_quants, make_qx_quants and nearest_int.
+ * Every fp32 operation is rounded on its own in the reference's order, so the bytes are a function of the input: they equal a
+ * plain-C restatement compiled with -ffp-contract=off, bit for bit, for every finite source.  Parity with a llama-quantize
+ * binary is NOT verified (see DESIGN.md section 8); a build that contracts multiply-adds into FMAs can differ in a scale's last
+ * bit.  Any other ggml_type: GGUFB200_E_TYPE; ggufb200_supported(t, GGUFB200_OP_QUANTIZE_K) lists exactly these five.
+ *   src        n_blocks * 256 contiguous values of src_dtype (0 fp16 / 1 bf16 / 2 fp32), aligned to one value
+ *              (GGUFB200_E_ALIGN otherwise)
+ *   n_blocks   super-blocks to write
+ *   packed     n_blocks * type_size bytes (84 / 110 / 144 / 176 / 210), any alignment
+ *   flags      0; any other bit: GGUFB200_E_UNSUPPORTED (reserved)
+ * Launched like ggufb200_quantize: a following stable-source dequant or Linear on the same stream may consume the packed bytes
+ * without any other synchronisation.
+ *   stream     a cudaStream_t
+ */
+int ggufb200_quantize_k(int ggml_type, const void *src, int src_dtype, int64_t n_blocks, void *packed, int flags, void *stream);
 
 /*
  * Integer unpack only (test/debug surface for the "bit-exact integer unpack" contract):

@@ -1,10 +1,12 @@
-"""GPU quantiser (ggufb200_quantize) throughput and a full Flux-shape conversion.
+"""GPU quantiser (ggufb200_quantize, ggufb200_quantize_k) throughput and a full Flux-shape conversion.
 
 1. Kernel GB/s per type and source dtype over the seven Flux Linear shapes: algorithmic bytes = source bytes read + packed bytes
-   written, CUDA events around `--iters` launches that rotate over enough copies of the tensor to spill L2.
+   written, CUDA events around `--iters` launches that rotate over enough copies of the tensor to spill L2.  The K types
+   (Q6_K ... Q2_K, ggufb200_quantize_k) are compute-bound: their rows report the same source-plus-output GB/s and the time.
 2. Baseline: gguf-py's numpy `gguf.quants.quantize` on the same tensors (fp32 input; one run per shape, `--numpy-shapes`).
-3. A full convert of a random Flux-shape checkpoint (19 double + 38 single blocks, bf16, `--blocks` to shorten) to `--qtype`,
-   the time split into read, quantise (including the copies to and from the GPU) and write.
+3. A full convert of a random Flux-shape checkpoint (19 double + 38 single blocks, bf16, `--blocks` to shorten) to each
+   `--qtype` (a type or a K mixture such as Q4_K_S), the time split into read, quantise (including the copies to and from the
+   GPU) and write.
 Prints the card name and power limit first; `--json PATH` also writes the rows."""
 import argparse
 import json
@@ -26,15 +28,17 @@ from bench_sd_linears import card  # noqa: E402
 Q = gguf.GGMLQuantizationType
 SHAPES = [(3072, 3072), (9216, 3072), (12288, 3072), (3072, 12288), (18432, 3072), (21504, 3072), (3072, 15360)]
 TYPES = [Q.Q8_0, Q.Q5_1, Q.Q5_0, Q.Q4_1, Q.Q4_0, Q.BF16]
+K_TYPES = [Q.Q6_K, Q.Q5_K, Q.Q4_K, Q.Q3_K, Q.Q2_K]
 SRC = {"f32": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16}
 
 
-def kernel_rows(L, lib, iters):
+def kernel_rows(L, lib, iters, types):
     dev = torch.device("cuda:0")
     stream = torch.cuda.current_stream(dev).cuda_stream
     rows = []
     for name, dt in SRC.items():
-        for qt in TYPES:
+        for qt in types:
+            entry = L.ggufb200_quantize_k if qt in K_TYPES else L.ggufb200_quantize
             bs, ts = gguf.GGML_QUANT_SIZES[qt]
             moved = total_s = 0.0
             for N, K in SHAPES:
@@ -43,7 +47,7 @@ def kernel_rows(L, lib, iters):
                 xs = [(torch.randn(N, K, device=dev) * 0.02).to(dt) for _ in range(copies)]
                 outs = [torch.empty(n // bs * ts, dtype=torch.uint8, device=dev) for _ in range(copies)]
                 code = {torch.float16: lib.F16, torch.bfloat16: lib.BF16, torch.float32: lib.F32}[dt]
-                launch = lambda i: L.ggufb200_quantize(int(qt), xs[i % copies].data_ptr(), code, n // bs, outs[i % copies].data_ptr(), 0, stream)
+                launch = lambda i: entry(int(qt), xs[i % copies].data_ptr(), code, n // bs, outs[i % copies].data_ptr(), 0, stream)
                 for i in range(copies):
                     assert launch(i) == 0
                 torch.cuda.synchronize()
@@ -60,7 +64,7 @@ def kernel_rows(L, lib, iters):
                 total_s += sec
                 del xs, outs
             print(f"{name:>5} {qt.name:>5}: " + " ".join(f"{r['GB/s']:7.0f}" for r in rows[-len(SHAPES):])
-                  + f"   all shapes {moved / total_s / 1e9:7.0f} GB/s", flush=True)
+                  + f"   all shapes {moved / total_s / 1e9:7.0f} GB/s, {total_s * 1e3:8.2f} ms", flush=True)
     return rows
 
 
@@ -123,7 +127,8 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--numpy-shapes", type=int, default=2)
-    ap.add_argument("--qtype", default="Q8_0")
+    ap.add_argument("--qtype", nargs="+", default=["Q8_0"], help="conversion targets: types or K mixtures")
+    ap.add_argument("--types", nargs="+", default=[q.name for q in TYPES + K_TYPES], help="kernel rows for these types")
     ap.add_argument("--blocks", type=int, nargs=2, default=[19, 38], metavar=("DOUBLE", "SINGLE"))
     ap.add_argument("--tmp", default=None, help="directory for the converted checkpoint (default: a temporary directory)")
     ap.add_argument("--json", default=None)
@@ -134,9 +139,10 @@ def main():
     info = card()
     print(json.dumps(info), flush=True)
     print("kernel GB/s per shape " + " ".join(f"{N}x{K}" for N, K in SHAPES), flush=True)
-    out = {"card": info, "kernel": kernel_rows(lib.lib(), lib, args.iters), "numpy": numpy_rows(args.numpy_shapes)}
+    types = [Q[t] for t in args.types]
+    out = {"card": info, "kernel": kernel_rows(lib.lib(), lib, args.iters, types), "numpy": numpy_rows(args.numpy_shapes)}
     with tempfile.TemporaryDirectory(dir=args.tmp) as tmp:
-        out["convert"] = convert_row(args.qtype, args.blocks[0], args.blocks[1], tmp)
+        out["convert"] = [convert_row(q, args.blocks[0], args.blocks[1], tmp) for q in args.qtype]
     if args.json:
         with open(args.json, "w") as f:
             json.dump(out, f, indent=1)

@@ -3,7 +3,10 @@
     python tools/convert.py --src flux1-dev.safetensors                      # F16 / BF16 file, as the reference's convert.py
     python tools/convert.py --src flux1-dev.safetensors --qtype Q8_0         # quantised in the same run (needs a CUDA device)
 
---qtype: F16, BF16, Q8_0, Q5_1, Q5_0, Q4_1 or Q4_0.  See comfyui-gguf_b200/convert.py for the type policy.
+    python tools/convert.py --src flux1-dev.safetensors --qtype Q4_K_S       # a llama-quantize K mixture, also on the GPU
+
+--qtype: F16, BF16, Q8_0, Q5_1, Q5_0, Q4_1 or Q4_0, or one of llama-quantize's K mixtures Q2_K, Q3_K_S, Q3_K_M, Q3_K_L, Q4_K_S,
+Q4_K_M, Q5_K_S, Q5_K_M or Q6_K.  See comfyui-gguf_b200/convert.py for the type policy.
 """
 import argparse
 import logging
@@ -20,7 +23,7 @@ def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--src", required=True, help="source checkpoint")
     ap.add_argument("--dst", help="output .gguf (default: <src>-<type>.gguf; '{ftype}' is replaced by the type name)")
-    ap.add_argument("--qtype", choices=sorted(convert.QTYPES), help="quantise to this type (default: the F16 / BF16 file)")
+    ap.add_argument("--qtype", choices=sorted(convert.QTYPES) + sorted(convert.KQUANT_MIXTURES), help="quantise to this type (default: the F16 / BF16 file)")
     ap.add_argument("--overwrite", action="store_true", help="replace an existing output file")
     args = ap.parse_args(argv)
     if not os.path.isfile(args.src):
