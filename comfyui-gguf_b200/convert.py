@@ -23,6 +23,11 @@ convert_file() writes in one pass what the reference's two steps write:
       and Q4_K_S depends on how many attention-value tensors came before, in file order); a tensor whose rows are not a
       multiple of 256 then becomes F16, even when stage 1 holds BF16.  The K bytes come from quantize_k_tensor.
 Tensors are written in input order with their full shapes.
+
+convert_gguf_file() is the second step alone, for a GGUF input (what the patched llama-quantize takes): an F16 / BF16 / F32
+stage-1 file of this module or of the reference, a stable-diffusion.cpp file without an architecture field, or an already
+quantised file (requantised on the GPU only when asked).  The same rules plan its tensors (plan_gguf), so a stage-1 file written
+here converts to the very bytes convert_file writes from the checkpoint.
 """
 from __future__ import annotations
 
@@ -34,6 +39,8 @@ from dataclasses import dataclass, field
 import gguf
 import numpy as np
 import torch
+
+from .dequant import FALLBACK_QTYPES, SUPPORTED_QTYPES
 
 _Q = gguf.GGMLQuantizationType
 
@@ -281,15 +288,18 @@ def plan_tensors(state_dict: dict, arch: Arch, qtype=None) -> list:
         orig = None
         if reshape:
             orig, shape = shape, (t.numel() // 256, 256)
-        if isinstance(qtype, KMixture):
-            final = stage1
-            if quantisable(key, stage1, shape, arch):
-                final = kquant_type(key, shape, qtype, n_attn_v)
-                n_attn_v += is_attn_v(key)        # counted before the row check, as the patch does
-        else:
-            final = stage2_type(key, stage1, shape, arch, qtype)
+        final, n_attn_v = _final_type(key, stage1, shape, arch, qtype, n_attn_v)
         plans.append(TensorPlan(key, shape, orig, stage1, final))
     return plans
+
+
+def _final_type(key: str, stage1: _Q, shape, arch: Arch, qtype, n_attn_v: int):
+    """(final type of one tensor, the attention-value count after it) for `qtype`: None, a type, or a KMixture."""
+    if isinstance(qtype, KMixture):
+        if not quantisable(key, stage1, shape, arch):
+            return stage1, n_attn_v
+        return kquant_type(key, shape, qtype, n_attn_v), n_attn_v + is_attn_v(key)   # counted before the row check, as the patch does
+    return stage2_type(key, stage1, shape, arch, qtype), n_attn_v
 
 
 def _stage1_values(t: torch.Tensor, stage1: _Q) -> torch.Tensor:
@@ -334,6 +344,33 @@ def tensor_bytes(t: torch.Tensor, plan: TensorPlan, device=None) -> np.ndarray:
     return packed.cpu().numpy().reshape(-1)
 
 
+def _parse_qtype(qtype):
+    """None, a type of FILE_TYPES, or a KMixture, from a name of QTYPES / KQUANT_MIXTURES, a type, or a KMixture."""
+    if isinstance(qtype, str):
+        if qtype.upper() in KQUANT_MIXTURES:
+            return KQUANT_MIXTURES[qtype.upper()]
+        if qtype.upper() not in QTYPES:
+            raise ValueError(f"unsupported qtype {qtype!r}: one of {', '.join(list(QTYPES) + list(KQUANT_MIXTURES))}")
+        return QTYPES[qtype.upper()]
+    if qtype is not None and not isinstance(qtype, KMixture):
+        qtype = _Q(qtype)
+        if qtype not in FILE_TYPES:
+            raise ValueError(f"unsupported qtype {qtype.name}: one of {', '.join(QTYPES)}")
+    return qtype
+
+
+def _dst_path(src_path: str, dst_path: str | None, name: str, overwrite: bool) -> str:
+    """dst_path, or `<src without extension>-<name>.gguf`, with `{ftype}` replaced by `name`; an existing file is refused unless
+    `overwrite`."""
+    if dst_path is None:
+        dst_path = f"{os.path.splitext(src_path)[0]}-{name}.gguf"
+    elif "{ftype}" in dst_path:
+        dst_path = dst_path.replace("{ftype}", name)
+    if os.path.exists(dst_path) and not overwrite:
+        raise FileExistsError(f"{dst_path} exists (pass overwrite=True / --overwrite to replace it)")
+    return dst_path
+
+
 @dataclass
 class ConvertResult:
     path: str
@@ -345,17 +382,7 @@ class ConvertResult:
 def convert_state_dict(state_dict: dict, dst_path: str, qtype=None, arch: Arch | None = None, device=None) -> ConvertResult:
     """Write the GGUF file of a prefix-stripped state dict (see the module docstring).  `qtype`: None (the F16 / BF16 file),
     one of QTYPES' names or values, or one of KQUANT_MIXTURES' names (or a KMixture)."""
-    if isinstance(qtype, str):
-        if qtype.upper() in KQUANT_MIXTURES:
-            qtype = KQUANT_MIXTURES[qtype.upper()]
-        elif qtype.upper() not in QTYPES:
-            raise ValueError(f"unsupported qtype {qtype!r}: one of {', '.join(list(QTYPES) + list(KQUANT_MIXTURES))}")
-        else:
-            qtype = QTYPES[qtype.upper()]
-    elif qtype is not None and not isinstance(qtype, KMixture):
-        qtype = _Q(qtype)
-        if qtype not in FILE_TYPES:
-            raise ValueError(f"unsupported qtype {qtype.name}: one of {', '.join(QTYPES)}")
+    qtype = _parse_qtype(qtype)
     arch = arch or detect_arch(state_dict.keys())
     too_long = [k for k in state_dict if len(k) > MAX_TENSOR_NAME_LENGTH]
     if too_long:
@@ -411,12 +438,221 @@ def convert_file(src_path: str, dst_path: str | None = None, qtype=None, overwri
     else:
         dtypes = [t.dtype for t in sd.values()]
         name = "BF16" if dtypes and max(set(dtypes), key=dtypes.count) == torch.bfloat16 else "F16"
-    if dst_path is None:
-        dst_path = f"{os.path.splitext(src_path)[0]}-{name}.gguf"
-    elif "{ftype}" in dst_path:
-        dst_path = dst_path.replace("{ftype}", name)
-    if os.path.exists(dst_path) and not overwrite:
-        raise FileExistsError(f"{dst_path} exists (pass overwrite=True / --overwrite to replace it)")
+    dst_path = _dst_path(src_path, dst_path, name, overwrite)
     result = convert_state_dict(sd, dst_path, qtype, arch, device)
     result.seconds["read"] = read
     return result
+
+
+# ------------------------------------------------------------------ GGUF sources: llama-quantize's step on the GPU
+_STAGE1_DTYPES = {_Q.F32: torch.float32, _Q.F16: torch.float16, _Q.BF16: torch.bfloat16}
+# the packed types a source tensor may hold and still be quantised again: K1's (BF16 aside, a stage-1 type) and the fallback's
+REQUANT_TYPES = tuple(q for q in SUPPORTED_QTYPES if q != _Q.BF16) + FALLBACK_QTYPES
+# the reference's stage 1 leaves these architectures' 5-D tensors in a side file, fix_5d_tensors_<arch>.safetensors
+ND_SIDE_FILE_ARCHES = ("hyvid", "wan")
+DIFFUSION_PREFIX = "model.diffusion_model."
+_KV_FILE_TYPE = gguf.Keys.General.FILE_TYPE
+_KV_QUANT_VERSION = gguf.Keys.General.QUANTIZATION_VERSION
+
+
+@dataclass
+class GGUFSource:
+    """A GGUF file opened for conversion.  `rule_names[i]` is the name the type rules see for tensor i: its name, without
+    `model.diffusion_model.` when any tensor has that prefix (None for the others, which are copied as they are), as the loader
+    strips it.  `arch_field`: general.architecture, None for a stable-diffusion.cpp file."""
+    path: str
+    reader: gguf.GGUFReader
+    arch: Arch
+    arch_field: str | None
+    rule_names: list
+
+
+def open_gguf_source(path: str) -> GGUFSource:
+    """Open `path` (memory-mapped: tensor bytes are read when a tensor is converted) and find its architecture: the
+    general.architecture field, or, without one, the tensor names as loader._check_arch recognises them."""
+    reader = gguf.GGUFReader(path)
+    field = reader.get_field(gguf.Keys.General.ARCHITECTURE)
+    arch_field = field.contents() if field is not None else None
+    names = [t.name for t in reader.tensors]
+    if any(n.startswith(DIFFUSION_PREFIX) for n in names):
+        rule_names = [n[len(DIFFUSION_PREFIX):] if n.startswith(DIFFUSION_PREFIX) else None for n in names]
+    else:
+        rule_names = names
+    if arch_field is None:
+        arch = detect_arch(n for n in rule_names if n is not None)
+        logging.info(f"* No architecture field: stable-diffusion.cpp file of architecture {arch.name}")
+    elif arch_field in ARCH_BY_NAME:
+        arch = ARCH_BY_NAME[arch_field]
+    else:
+        raise ValueError(f"{path}: unsupported architecture {arch_field!r} (one of {', '.join(ARCH_BY_NAME)})")
+    return GGUFSource(path, reader, arch, arch_field, rule_names)
+
+
+def _orig_shapes(reader) -> dict:
+    pre = "comfy.gguf.orig_shape."
+    return {k[len(pre):]: tuple(int(d) for d in f.contents()) for k, f in reader.fields.items() if k.startswith(pre)}
+
+
+def plan_gguf(src: GGUFSource, qtype, fix_5d: dict | None = None) -> list:
+    """Every written tensor's plan, in output order, for `qtype` (a type or a KMixture).  The source tensor's type plays the
+    part of stage 1 and its stored shape is the shape; a packed source tensor is ruled on as the F16 tensor it was made from,
+    and keeps its type where the rules leave it alone.  `fix_5d` ({name: tensor}): tensors merged as F32, each right after the
+    `.bias` it belongs to, the rest at the end (where the reference's fix_5d_tensors.py puts them)."""
+    orig = _orig_shapes(src.reader)
+    side = dict(fix_5d or {})
+    clash = [k for k in side if k in {t.name for t in src.reader.tensors}]
+    if clash:
+        raise ValueError(f"{src.path} already holds {', '.join(clash)}: nothing to merge from the 5-D tensor file")
+    plans, n_attn_v = [], 0
+
+    def merge(key):
+        t = side.pop(key)
+        plans.append(TensorPlan(key, tuple(int(d) for d in t.shape), None, _Q.F32, _Q.F32))
+
+    for t, key in zip(src.reader.tensors, src.rule_names):
+        source = _Q(t.tensor_type)
+        shape = tuple(int(d) for d in reversed(t.shape.tolist()))
+        final = source
+        if key is not None and (source in _STAGE1_DTYPES or source in REQUANT_TYPES):
+            rule = source if source in _STAGE1_DTYPES else _Q.F16
+            final, n_attn_v = _final_type(key, rule, shape, src.arch, qtype, n_attn_v)
+            if not quantisable(key, rule, shape, src.arch):
+                final = source
+        plans.append(TensorPlan(t.name, shape, orig.get(t.name), source, final))
+        if t.name.replace(".bias", ".weight") in side:
+            merge(t.name.replace(".bias", ".weight"))
+    for key in list(side):
+        merge(key)
+    return plans
+
+
+def missing_nd_weights(src: GGUFSource) -> list:
+    """The `.weight` names a reference stage-1 file of an ND_SIDE_FILE_ARCHES architecture lacks: a `.bias` without one."""
+    if src.arch.name not in ND_SIDE_FILE_ARCHES:
+        return []
+    names = {t.name for t in src.reader.tensors}
+    return [n[:-len(".bias")] + ".weight" for n in names if n.endswith(".bias") and n[:-len(".bias")] + ".weight" not in names]
+
+
+def needs_gpu(plan: TensorPlan) -> bool:
+    """Whether `plan` runs on the GPU: the quantiser, or a packed source tensor decoded to be written as another type."""
+    return needs_quantiser(plan) or (plan.stage1 in REQUANT_TYPES and plan.qtype != plan.stage1)
+
+
+def _gguf_kv(src: GGUFSource, file_type) -> list:
+    """(key, value, type, array item type) of every field the output carries: the source's, in source order; general.
+    quantization_version and general.file_type set (appended when absent) as llama-quantize sets them, except in a file
+    without an architecture field, whose fields stay exactly as they are so that it still loads in compatibility mode."""
+    kv = {}
+    for name, f in src.reader.fields.items():
+        if name.startswith("GGUF."):                # the header's version and counts, not fields
+            continue
+        vtype = f.types[0]
+        if vtype == gguf.GGUFValueType.ARRAY and len(f.types) != 2:
+            raise ValueError(f"{src.path}: field {name!r} is an array of arrays, which this converter does not copy")
+        kv[name] = (f.contents(), vtype, f.types[1] if vtype == gguf.GGUFValueType.ARRAY else None)
+    if src.arch_field is not None:
+        kv[_KV_QUANT_VERSION] = (gguf.GGML_QUANT_VERSION, gguf.GGUFValueType.UINT32, None)
+        kv[_KV_FILE_TYPE] = (int(file_type), gguf.GGUFValueType.UINT32, None)
+    return [(k, *v) for k, v in kv.items()]
+
+
+def _gpu_device(device):
+    if device is None:
+        device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
+    return torch.device(device)
+
+
+def gguf_tensor_bytes(raw: np.ndarray, plan: TensorPlan, device=None) -> np.ndarray:
+    """The bytes `plan` writes for a source tensor whose stored bytes are `raw` (uint8, writable): the same bytes when the
+    type stays; F32 / F16 / BF16 values through tensor_bytes; a packed tensor decoded on the GPU to fp32 (K1 with fp32 math
+    and output, or the fallback dequant) and encoded there."""
+    if plan.qtype == plan.stage1:
+        return raw
+    if plan.stage1 in _STAGE1_DTYPES:
+        return tensor_bytes(torch.from_numpy(raw).view(_STAGE1_DTYPES[plan.stage1]).reshape(plan.shape), plan, device)
+    from .dequant import dequantize, dequantize_fallback
+    from .quantize import quantize_k_tensor, quantize_tensor
+    packed = torch.from_numpy(raw).to(_gpu_device(device))
+    if plan.stage1 in FALLBACK_QTYPES:
+        v = dequantize_fallback(packed, plan.stage1, plan.shape)
+    else:
+        v = dequantize(packed, plan.stage1, plan.shape, dtype=torch.float32, out_dtype=torch.float32)
+    if plan.qtype == _Q.F16:
+        out = v.to(torch.float16).reshape(-1).view(torch.uint8)
+    elif plan.qtype in KQUANT_TYPES:
+        out = quantize_k_tensor(v, plan.qtype)
+    else:
+        out = quantize_tensor(v, plan.qtype)
+    return out.cpu().numpy().reshape(-1)
+
+
+def convert_gguf_file(src_path: str, dst_path: str | None = None, qtype=None, overwrite: bool = False,
+                      allow_requantize: bool = False, fix_5d: str | None = None, device=None) -> ConvertResult:
+    """Quantise the GGUF file at `src_path` to `qtype` (required: one of QTYPES' or KQUANT_MIXTURES' names, a type or a
+    KMixture), as llama-quantize with the image-model patch does; dst_path / overwrite as convert_file.
+
+    The tensors are planned by the rules of plan_tensors (plan_gguf).  An F16 / BF16 tensor the rules quantise is quantised
+    from its stored values, so a stage-1 file this module wrote converts to exactly the file convert_file writes from the
+    checkpoint.  Every tensor whose type stays is copied byte for byte.  A packed source tensor planned as another type is
+    refused (`requantizing from type X is disabled`) unless `allow_requantize`, and is then decoded and encoded on the GPU.
+    `fix_5d`: the side file of the reference's stage 1 for hyvid / wan (fix_5d_tensors_<arch>.safetensors), merged as F32;
+    a hyvid / wan file that lacks a 5-D weight is refused without it.  A stable-diffusion.cpp file (no general.architecture)
+    keeps its tensor names and fields as they are."""
+    t0 = time.perf_counter()
+    qtype = _parse_qtype(qtype)
+    if qtype is None:
+        raise ValueError(f"convert_gguf_file needs a qtype: one of {', '.join(list(QTYPES) + list(KQUANT_MIXTURES))}")
+    src = open_gguf_source(src_path)
+    logging.info(f"* Architecture of the GGUF input: {src.arch.name}")
+    side = None
+    if fix_5d is not None:
+        from safetensors.torch import load_file
+        side = load_file(fix_5d)
+    else:
+        missing = missing_nd_weights(src)
+        if missing:
+            raise ValueError(f"{src_path} lacks {', '.join(repr(k) for k in sorted(missing))}: the reference's stage 1 leaves "
+                             f"{src.arch.name}'s 5-D tensors in fix_5d_tensors_{src.arch.name}.safetensors; pass that file as "
+                             "fix_5d=PATH (--fix-5d PATH) to merge it")
+    plans = plan_gguf(src, qtype, side)
+    requant = [p for p in plans if p.stage1 in REQUANT_TYPES and p.qtype != p.stage1]
+    if requant and not allow_requantize:
+        raise ValueError(f"requantizing from type {requant[0].stage1.name} is disabled (tensor {requant[0].key!r}; pass "
+                         "allow_requantize=True / --allow-requantize to decode and quantise it again)")
+    dst_path = _dst_path(src_path, dst_path, qtype.name, overwrite)
+    if any(needs_gpu(p) for p in plans) and device is None and not torch.cuda.is_available():
+        raise NotImplementedError(f"quantising to {qtype.name} runs on the GPU and no CUDA device is visible")
+    file_type = qtype.file_type if isinstance(qtype, KMixture) else FILE_TYPES[qtype]
+
+    writer = gguf.GGUFWriter(path=None, arch=src.arch_field or "")
+    writer.kv_data[0].clear()                       # the source's fields, in source order, replace the writer's own
+    for key, val, vtype, sub in _gguf_kv(src, file_type):
+        writer.add_key_value(key, val, vtype, sub)
+        if key == gguf.Keys.General.ALIGNMENT:
+            writer.data_alignment = int(val)
+    for p in plans:
+        byte_shape = gguf.quant_shape_to_byte_shape(p.shape, p.qtype)
+        writer.add_tensor_info(p.key, byte_shape, np.dtype(np.uint8), int(np.prod(byte_shape, dtype=np.int64)), raw_dtype=p.qtype)
+    t_read, t_quant, t_write = time.perf_counter() - t0, 0.0, 0.0
+    writer.write_header_to_file(path=dst_path)
+    writer.write_kv_data_to_file()
+    writer.write_ti_data_to_file()
+    tensors = {t.name: t for t in src.reader.tensors}
+    for p in plans:
+        t0 = time.perf_counter()
+        if p.key in tensors:
+            t = tensors[p.key]
+            raw = np.array(src.reader.data[t.data_offset:t.data_offset + t.n_bytes])
+        else:
+            raw = side[p.key].to(torch.float32).contiguous().numpy().view(np.uint8).reshape(-1)
+        t1 = time.perf_counter()
+        data = gguf_tensor_bytes(raw, p, device)
+        t2 = time.perf_counter()
+        writer.write_tensor_data(data)
+        t_write += time.perf_counter() - t2
+        t_quant += t2 - t1
+        t_read += t1 - t0
+        logging.info(f"{p.key:<{MAX_TENSOR_NAME_LENGTH}} {p.stage1.name} --> {p.qtype.name}, shape = {p.shape}")
+    writer.close()
+    return ConvertResult(dst_path, src.arch, plans, {"read": t_read, "quantise": t_quant, "write": t_write})

@@ -7,6 +7,8 @@
 3. A full convert of a random Flux-shape checkpoint (19 double + 38 single blocks, bf16, `--blocks` to shorten) to each
    `--qtype` (a type or a K mixture such as Q4_K_S), the time split into read, quantise (including the copies to and from the
    GPU) and write.
+4. `--gguf`: the same checkpoint's stage-1 BF16 GGUF -> Q4_K_S, and a Q8_0 GGUF -> Q4_K_S with requantisation
+   (convert_gguf_file), each beside the direct conversion of the checkpoint to Q4_K_S, split the same way.
 Prints the card name and power limit first; `--json PATH` also writes the rows."""
 import argparse
 import json
@@ -123,14 +125,43 @@ def convert_row(qtype, blocks_double, blocks_single, tmp):
     return row
 
 
+def gguf_rows(blocks_double, blocks_single, tmp, qtype="Q4_K_S"):
+    """Direct checkpoint -> qtype, then stage-1 BF16 GGUF -> qtype and Q8_0 GGUF -> qtype (requantised), on one checkpoint."""
+    from safetensors.torch import save_file
+    conv = ge._sub("convert")
+    src = os.path.join(tmp, "flux.safetensors")
+    save_file(flux_checkpoint(blocks_double, blocks_single), src)
+    rows = []
+
+    def row(kind, res, src_path):
+        rows.append({"kind": kind, "qtype": qtype, "double_blocks": blocks_double, "single_blocks": blocks_single,
+                     "src_bytes": os.path.getsize(src_path), "dst_bytes": os.path.getsize(res.path),
+                     **{f"{k}_s": v for k, v in res.seconds.items()}})
+        print(f"{kind} -> {qtype} ({rows[-1]['src_bytes'] / 1e9:.1f} GB -> {rows[-1]['dst_bytes'] / 1e9:.2f} GB): "
+              + ", ".join(f"{k} {v:.2f} s" for k, v in res.seconds.items()) + f", total {sum(res.seconds.values()):.2f} s", flush=True)
+        os.remove(res.path)
+
+    row("safetensors bf16", conv.convert_file(src, os.path.join(tmp, "direct.gguf"), qtype=qtype, overwrite=True), src)
+    bf16 = conv.convert_file(src, os.path.join(tmp, "flux-BF16.gguf"), overwrite=True).path
+    os.remove(src)
+    row("GGUF BF16", conv.convert_gguf_file(bf16, os.path.join(tmp, "from-bf16.gguf"), qtype, overwrite=True), bf16)
+    q8 = conv.convert_gguf_file(bf16, os.path.join(tmp, "flux-Q8_0.gguf"), "Q8_0", overwrite=True).path
+    os.remove(bf16)
+    row("GGUF Q8_0, requantised", conv.convert_gguf_file(q8, os.path.join(tmp, "from-q8.gguf"), qtype, overwrite=True,
+                                                        allow_requantize=True), q8)
+    os.remove(q8)
+    return rows
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--numpy-shapes", type=int, default=2)
     ap.add_argument("--qtype", nargs="+", default=["Q8_0"], help="conversion targets: types or K mixtures")
-    ap.add_argument("--types", nargs="+", default=[q.name for q in TYPES + K_TYPES], help="kernel rows for these types")
+    ap.add_argument("--types", nargs="*", default=[q.name for q in TYPES + K_TYPES], help="kernel rows for these types")
     ap.add_argument("--blocks", type=int, nargs=2, default=[19, 38], metavar=("DOUBLE", "SINGLE"))
     ap.add_argument("--tmp", default=None, help="directory for the converted checkpoint (default: a temporary directory)")
+    ap.add_argument("--gguf", action="store_true", help="also time the GGUF-input conversions (step 4)")
     ap.add_argument("--json", default=None)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_quantize needs a GPU"
@@ -143,6 +174,8 @@ def main():
     out = {"card": info, "kernel": kernel_rows(lib.lib(), lib, args.iters, types), "numpy": numpy_rows(args.numpy_shapes)}
     with tempfile.TemporaryDirectory(dir=args.tmp) as tmp:
         out["convert"] = [convert_row(q, args.blocks[0], args.blocks[1], tmp) for q in args.qtype]
+        if args.gguf:
+            out["gguf"] = gguf_rows(args.blocks[0], args.blocks[1], tmp)
     if args.json:
         with open(args.json, "w") as f:
             json.dump(out, f, indent=1)
