@@ -431,6 +431,15 @@ def _patch_entries(tensor):
 _ADAPTER_KINDS = {"LoRAAdapter": "lora", "LoHaAdapter": "loha", "LoKrAdapter": "lokr"}
 
 
+def _entry_tensors(entry):
+    """The tensors of a patch entry's payload ((kind, payload) or an adapter's `.weights`)."""
+    value = entry[1] if len(entry) > 1 else None
+    payload = getattr(value, "weights", None)
+    if payload is None and isinstance(value, (tuple, list)) and len(value) == 2:
+        payload = value[1]
+    return [t for t in (payload or ()) if torch.is_tensor(t)] if isinstance(payload, (tuple, list)) else []
+
+
 def _mat(t):
     return torch.is_tensor(t) and t.dim() == 2
 
@@ -1390,9 +1399,30 @@ class GGMLOps(comfy_ops.manual_cast):
         lora_in_kernel = True
 
         def _lora_operands(self, terms, dev, dtype):
-            """`lora_kernel_operands` of `_lora_terms`, cached per patch set, device and activation dtype."""
+            """`lora_kernel_operands` of `_lora_terms`, cached per patch set, device and activation dtype; None when U = scale * up
+            does not fit fp16 (or down the activation dtype): the side GEMMs, whose U is in the activation dtype, serve those."""
             key = tuple((float(scale), band, _tensor_key(up), _tensor_key(down)) for scale, up, down, band in terms) + (str(dev), dtype)
-            return _cached(self, "_gg_lora", key, lambda: lora_kernel_operands(terms, *self.weight.tensor_shape, dtype, dev))
+
+            def build():
+                down_pad, u_pad, tiles = lora_kernel_operands(terms, *self.weight.tensor_shape, dtype, dev)
+                return (down_pad, u_pad, tiles) if bool(torch.isfinite(u_pad).all()) and bool(torch.isfinite(down_pad).all()) else None
+            return _cached(self, "_gg_lora", key, build)
+
+        def _patches_finite(self, dev, dtype, terms):
+            """False when a tensor of the weight's patch entries holds NaN / Inf, or a LoRA-form term's scale * up or down (the
+            side GEMMs' operands) does not fit the activation dtype.  Such a patch set takes the two-step route: a factorised
+            evaluation sums the rank terms before an infinity meets them (an Inf in up is NaN in the reference's x W'^T, +-Inf in
+            t u^T; a NaN in a banded term's factor would reach the rows of its tile outside the band), so only the reference's
+            own arithmetic gives its NaN / Inf pattern.  Cached per patch set, device and activation dtype."""
+            tensors = [t for entry in _patch_entries(self.weight) for t in _entry_tensors(entry)]
+            key = tuple(map(_tensor_key, tensors)) + tuple(float(s) for s, *_r in terms or ()) + (str(dev), dtype)
+
+            def build():
+                if not all(bool(torch.isfinite(t).all()) for t in tensors):
+                    return False
+                return all(bool(torch.isfinite((up.to(device=dev, dtype=torch.float32) * scale).to(dtype)).all())
+                           and bool(torch.isfinite(down.to(device=dev, dtype=dtype)).all()) for scale, up, down, _band in terms or ())
+            return _cached(self, "_gg_finite", key, build)
 
         def _lycoris_terms(self, dev):
             """For a patch list with LoHa / LoKr entries (`lycoris_terms`, any mix with LoRA): `lycoris_operands` on `dev`, cached
@@ -1530,6 +1560,8 @@ class GGMLOps(comfy_ops.manual_cast):
                         terms, kron = lycoris
                 if terms is None and not grad:
                     dora = self._dora_terms()                          # tried after the LoRA and LyCORIS recognisers declined
+                if (terms or kron is not None or dora is not None) and not self._patches_finite(dev, input.dtype, terms):
+                    terms, kron, dora = None, None, None                # non-finite factors: the two-step route
                 if terms is not None or dora is not None:
                     w = self.weight
                     qtype, (N, K) = w.tensor_type, w.tensor_shape      # plain Python attributes: no subclass dispatch
@@ -1585,9 +1617,11 @@ class GGMLOps(comfy_ops.manual_cast):
                             algo = _lib.ALGO_FUSED_TMEM | exact
                         if (terms and not grad and self._takes_lora_kblocks(qtype, N, K, math, spans)
                                 and sum(d.shape[0] for _s, _u, d, _b in terms) <= LORA_KERNEL_MAX_RANK):
-                            down_pad, u_pad, tiles = self._lora_operands(terms, dev, input.dtype)
-                            lora = (linear_dense(input.reshape(-1, K), down_pad), u_pad, tiles)       # T = x * down^T, [M, 64 J]
-                            return _launch_linear(input, wraw, qtype, N, K, b, math, _lib.ALGO_FUSED_TMEM | exact, spans, lora)
+                            operands = self._lora_operands(terms, dev, input.dtype)
+                            if operands is not None:
+                                down_pad, u_pad, tiles = operands
+                                lora = (linear_dense(input.reshape(-1, K), down_pad), u_pad, tiles)       # T = x * down^T, [M, 64 J]
+                                return _launch_linear(input, wraw, qtype, N, K, b, math, _lib.ALGO_FUSED_TMEM | exact, spans, lora)
 
                         def run():
                             return _launch_linear(input, wraw, qtype, N, K, b, math, algo, spans)
